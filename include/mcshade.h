@@ -213,6 +213,29 @@ int mcs_interpolate_fwd(const float *attr, int64_t attr_batch_stride, int32_t V,
 int mcs_interpolate_bwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
                         int32_t B, int32_t H, int32_t W, const float *d_out, float *d_attr, mcs_stream stream);
 
+/* ---- geometry gradients through the G-buffer: the silhouette term of geometry/dlmesh.py:75 (alpha of render_mesh's composite_buffer,
+ *      render/render.py:290, where dr.antialias runs on every buffer) needs d rast / d pos.  pos: clip-space vertices [V,4]
+ *      (pos_batch_stride 0) or [B,V,4] (stride V*4), fp32 contiguous; it must equal mtx * (verts, 1) for the vertices the BVH was built from.
+ *      d_pos (same layout as pos) must be zeroed by the caller and receives float atomics; z and the id channel carry no gradient.
+ *   rasterize_bwd: d_rast [B,H,W,4] -> d_pos through the perspective-correct barycentrics of pos (derivation in csrc/raster.cu).
+ *   interpolate_bwd_rast: as mcs_interpolate_bwd, plus d_rast [B,H,W,4] = (sum_c g (A0 - A2), sum_c g (A1 - A2), 0, 0) written for every
+ *      pixel; d_attr may be null (no attribute gradient).
+ *   aa_topology: adj int32 [T,3], adj[t,k] = the triangle across edge (tri[t,k], tri[t,(k+1)%3]), -1 boundary, -2 three or more triangles;
+ *      workspace: mcs_aa_topology_workspace_bytes(T) bytes, 8-byte aligned, device memory, contents ignored on entry.
+ *   antialias: pixel-pair analytic antialiasing of color [B,H,W,C] (C >= 1, contiguous) given rast, pos, tris and adj; out [B,H,W,C].
+ *      The backward writes d_color [B,H,W,C] (overwritten, may be null) and adds into d_pos (may be null; not both null).
+ *      Semantics in csrc/raster.cu. */
+int mcs_rasterize_bwd(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B, int32_t H,
+                      int32_t W, const float *d_rast, float *d_pos, mcs_stream stream);
+int mcs_interpolate_bwd_rast(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
+                             int32_t B, int32_t H, int32_t W, const float *d_out, float *d_attr, float *d_rast, mcs_stream stream);
+int64_t mcs_aa_topology_workspace_bytes(int32_t T);
+int mcs_aa_topology(const int32_t *tris, int32_t T, void *workspace, int32_t *adj, mcs_stream stream);
+int mcs_antialias_fwd(const float *color, int32_t C, const float *rast, int32_t B, int32_t H, int32_t W, const float *pos, int64_t pos_batch_stride,
+                      int32_t V, const int32_t *tris, int32_t T, const int32_t *adj, float *out, mcs_stream stream);
+int mcs_antialias_bwd(const float *color, int32_t C, const float *rast, int32_t B, int32_t H, int32_t W, const float *pos, int64_t pos_batch_stride,
+                      int32_t V, const int32_t *tris, int32_t T, const int32_t *adj, const float *d_out, float *d_color, float *d_pos, mcs_stream stream);
+
 /* Nearest-texel fetch out[i,:] = tex[idx[i],:] (tex [T,C] contiguous, idx int64 [n]; out-of-range indices give zeros) and its scatter-add
  * backward into a caller-zeroed d_tex [T,C] (float atomics) -- the material look-up of the synthetic G-buffer producer. */
 int mcs_texel_fetch_fwd(const float *tex, int64_t T, int32_t C, const int64_t *idx, int64_t n, float *out, mcs_stream stream);

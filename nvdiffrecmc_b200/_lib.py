@@ -116,6 +116,12 @@ _SIGS = {
     "mcs_rasterize": ([_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
     "mcs_interpolate_fwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
     "mcs_interpolate_bwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
+    "mcs_interpolate_bwd_rast": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P], C.c_int),
+    "mcs_rasterize_bwd": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
+    "mcs_aa_topology_workspace_bytes": ([C.c_int32], C.c_int64),
+    "mcs_aa_topology": ([_P, C.c_int32, _P, _P, _P], C.c_int),
+    "mcs_antialias_fwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P], C.c_int),
+    "mcs_antialias_bwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 
@@ -143,7 +149,7 @@ def lib():
 # Count of OUR kernels launched through the C ABI (bench.py's gpu_launches claim).  optix_build_bvh launches eleven hand-written
 # kernels: bounds init, triangle bounds, Morton codes, radix sort (histogram + 4 passes), Karras topology, leaves + refit, node emission.
 LAUNCHES = collections.Counter()
-_KERNELS_PER_CALL = {"optix_build_bvh": 11, "bvh_export": 0, "update_pdf": 2, "rasterize": 2}
+_KERNELS_PER_CALL = {"optix_build_bvh": 11, "bvh_export": 0, "update_pdf": 2, "rasterize": 2, "antialias_topology": 2}
 
 
 def check(status, what):

@@ -1,25 +1,83 @@
-"""Primary visibility and attribute interpolation without a rasteriser (SURVEY section 8 row f2).
+"""Primary visibility, attribute interpolation and antialiasing without a rasteriser (SURVEY section 8 row f2).
 
-Stand-ins for the two nvdiffrast calls of the reference's G-buffer pass (render/render.py:208-234): `rasterize` traces one
-primary ray per pixel through the LBVH that `optix_build_bvh` already built for the shadow rays and returns nvdiffrast's
-`rast` tensor `(u, v, z/w, triangle_id + 1)`; `interpolate` evaluates vertex attributes at those barycentrics and is
-differentiable with respect to the attributes (float atomics in the backward pass, like dr.interpolate).  Screen-space
-derivatives (`rast_db`, `diff_attrs`) and antialiasing are not provided."""
+Stand-ins for the nvdiffrast calls of the reference's G-buffer pass (render/render.py:208-234) and of its compositing
+(`composite_buffer`, render.py:284-291): `rasterize` traces one primary ray per pixel through the LBVH that `optix_build_bvh`
+already built for the shadow rays and returns nvdiffrast's `rast` tensor `(u, v, z/w, triangle_id + 1)`; given the clip-space
+vertices `pos` it is differentiable with respect to them through the barycentrics.  `interpolate` evaluates vertex attributes at
+those barycentrics and is differentiable with respect to the attributes and to `rast`.  `antialias` is the pixel-pair analytic
+antialiasing of Laine et al. 2020, the only path from coverage (alpha) to vertex positions, so silhouette losses train the mesh;
+`antialias_topology` builds the edge adjacency it needs on the device.  Screen-space derivatives (`rast_db`, `diff_attrs`) are not
+provided."""
 import torch
 from . import _lib as L
 
 
-def rasterize(optix_ctx, mtx, resolution):
-    """mtx: [B,4,4] clip-space transform (clip = mtx @ (p, 1), the `mtx_in` of render_mesh, render.py:289-293);
-    resolution: (H, W).  Returns rast [B,H,W,4] fp32; a pixel whose ray hits nothing is all zeros."""
-    L.require_cuda(mtx)
-    if mtx.dim() != 3 or mtx.shape[1:] != (4, 4):
-        raise ValueError("rasterize: mtx must be [B,4,4]")
-    m = mtx.detach().to(torch.float32).contiguous()
+def _check_pos(pos, B, name):
+    if pos.dtype != torch.float32:
+        raise TypeError("%s: pos must be fp32 [V,4] or [B,V,4]" % name)
+    if not (pos.dim() == 2 and pos.shape[1] == 4) and not (pos.dim() == 3 and pos.shape[2] == 4):
+        raise ValueError("%s: pos must be [V,4] or [B,V,4], got %s" % (name, tuple(pos.shape)))
+    if pos.dim() == 3 and pos.shape[0] != B:
+        raise ValueError("%s: pos batch %d does not match %d" % (name, pos.shape[0], B))
+    V = pos.shape[-2]
+    return V, (V * 4 if pos.dim() == 3 else 0)
+
+
+def _check_tri(tri, name, what="tri"):
+    if tri.dtype != torch.int32:
+        raise TypeError("%s: %s must be int32 [T,3]" % (name, what))
+    if tri.dim() != 2 or tri.shape[1] != 3 or tri.shape[0] == 0:
+        raise ValueError("%s: %s must be a non-empty [T,3], got %s" % (name, what, tuple(tri.shape)))
+
+
+def _rasterize_launch(optix_ctx, m, resolution):
     B, (H, W) = m.shape[0], resolution
     rast = torch.empty(B, H, W, 4, dtype=torch.float32, device=m.device)
     L.check(L.lib().mcs_rasterize(optix_ctx.cpp_wrapper, m.data_ptr(), B, H, W, rast.data_ptr(), L.stream_ptr()), "rasterize")
     return rast
+
+
+class _rasterize_func(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pos, tri, optix_ctx, m, resolution):
+        rast = _rasterize_launch(optix_ctx, m, resolution)
+        ctx.save_for_backward(pos, tri, rast)
+        return rast
+
+    @staticmethod
+    def backward(ctx, d_rast):
+        pos, tri, rast = ctx.saved_tensors
+        B, H, W = rast.shape[0], rast.shape[1], rast.shape[2]
+        d_pos = torch.zeros_like(pos)
+        g = d_rast.to(torch.float32).contiguous()
+        V = pos.shape[-2]
+        L.check(L.lib().mcs_rasterize_bwd(pos.data_ptr(), V * 4 if pos.dim() == 3 else 0, V, tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W,
+                                          g.data_ptr(), d_pos.data_ptr(), L.stream_ptr()), "rasterize (backward)")
+        return d_pos, None, None, None, None
+
+
+def rasterize(optix_ctx, mtx, resolution, pos=None, tri=None):
+    """mtx: [B,4,4] clip-space transform (clip = mtx @ (p, 1), the `mtx_in` of render_mesh, render.py:289-293);
+    resolution: (H, W).  Returns rast [B,H,W,4] fp32; a pixel whose ray hits nothing is all zeros.
+
+    pos (clip-space vertices [V,4] or [B,V,4], fp32, equal to mtx @ (verts, 1) for the vertices the context's BVH was built from, e.g.
+    `ru.xfm_points(v_pos[None], mtx)`) and tri (int32 [T,3]) make the result differentiable with respect to pos: the forward is the
+    same ray-traced launch with a bit-identical output, and the backward maps d rast[...,0:2] to d pos through the perspective-correct
+    barycentrics of the clip-space triangle.  z/w and the id channel carry no gradient."""
+    L.require_cuda(mtx)
+    if mtx.dim() != 3 or mtx.shape[1:] != (4, 4):
+        raise ValueError("rasterize: mtx must be [B,4,4]")
+    m = mtx.detach().to(torch.float32).contiguous()
+    if pos is None:
+        if tri is not None:
+            raise ValueError("rasterize: tri is only used together with pos")
+        return _rasterize_launch(optix_ctx, m, resolution)
+    if tri is None:
+        raise ValueError("rasterize: pos needs tri")
+    L.require_cuda(pos, tri)
+    _check_pos(pos, m.shape[0], "rasterize")
+    _check_tri(tri, "rasterize")
+    return _rasterize_func.apply(pos.contiguous(), tri.contiguous(), optix_ctx, m, resolution)
 
 
 class _interpolate_func(torch.autograd.Function):
@@ -46,8 +104,15 @@ class _interpolate_func(torch.autograd.Function):
         batched = a.dim() == 3
         V, Cn = a.shape[-2], a.shape[-1]
         B, H, W = r.shape[0], r.shape[1], r.shape[2]
-        d_attr = torch.zeros_like(a)
         g = dout.to(torch.float32).contiguous()
+        if ctx.needs_input_grad[1]:
+            d_attr = torch.zeros_like(a) if ctx.needs_input_grad[0] else None
+            d_rast = torch.empty_like(r)
+            L.check(L.lib().mcs_interpolate_bwd_rast(a.data_ptr(), V * Cn if batched else 0, V, Cn, t.data_ptr(), t.shape[0], r.data_ptr(), B, H, W,
+                                                     g.data_ptr(), d_attr.data_ptr() if d_attr is not None else None, d_rast.data_ptr(),
+                                                     L.stream_ptr()), "interpolate (backward)")
+            return d_attr, d_rast, None
+        d_attr = torch.zeros_like(a)
         L.check(L.lib().mcs_interpolate_bwd(a.data_ptr(), V * Cn if batched else 0, V, Cn, t.data_ptr(), t.shape[0], r.data_ptr(), B, H, W,
                                             g.data_ptr(), d_attr.data_ptr(), L.stream_ptr()), "interpolate (backward)")
         return d_attr, None, None
@@ -56,6 +121,73 @@ class _interpolate_func(torch.autograd.Function):
 def interpolate(attr, rast, tri):
     """attr [V,C] or [B,V,C], rast from `rasterize`, tri int32 [T,3].  Returns (out [B,H,W,C], None) like dr.interpolate."""
     return _interpolate_func.apply(attr, rast, tri), None
+
+
+def antialias_topology(tri):
+    """Edge adjacency of a triangle list: int32 [T,3], entry k of triangle t is the triangle across edge (tri[t,k], tri[t,(k+1)%3]),
+    -1 on a boundary edge, -2 on an edge shared by three or more triangles.  Built on the device (hash of the undirected edge keys)
+    without a host sync; the result depends only on which triangles share each edge, not on the order they are inserted."""
+    L.require_cuda(tri)
+    _check_tri(tri, "antialias_topology")
+    t = tri.contiguous()
+    T = t.shape[0]
+    ws = torch.empty(int(L.lib().mcs_aa_topology_workspace_bytes(T)), dtype=torch.uint8, device=t.device)
+    adj = torch.empty(T, 3, dtype=torch.int32, device=t.device)
+    L.check(L.lib().mcs_aa_topology(t.data_ptr(), T, ws.data_ptr(), adj.data_ptr(), L.stream_ptr()), "antialias_topology")
+    return adj
+
+
+def _aa_args(color, rast, pos, tri, topology):
+    return (color.data_ptr(), color.shape[3], rast.data_ptr(), rast.shape[0], rast.shape[1], rast.shape[2], pos.data_ptr(),
+            pos.shape[-2] * 4 if pos.dim() == 3 else 0, pos.shape[-2], tri.data_ptr(), tri.shape[0], topology.data_ptr())
+
+
+class _antialias_func(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, color, pos, rast, tri, topology):
+        out = torch.empty_like(color)
+        L.check(L.lib().mcs_antialias_fwd(*_aa_args(color, rast, pos, tri, topology), out.data_ptr(), L.stream_ptr()), "antialias (forward)")
+        ctx.save_for_backward(color, pos, rast, tri, topology)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        color, pos, rast, tri, topology = ctx.saved_tensors
+        g = dout.to(torch.float32).contiguous()
+        d_color = torch.empty_like(color) if ctx.needs_input_grad[0] else None
+        d_pos = torch.zeros_like(pos) if ctx.needs_input_grad[1] else None
+        if d_color is None and d_pos is None:
+            return None, None, None, None, None
+        L.check(L.lib().mcs_antialias_bwd(*_aa_args(color, rast, pos, tri, topology), g.data_ptr(), d_color.data_ptr() if d_color is not None else None,
+                                          d_pos.data_ptr() if d_pos is not None else None, L.stream_ptr()), "antialias (backward)")
+        return d_color, d_pos, None, None, None
+
+
+def antialias(color, rast, pos, tri, topology=None):
+    """Analytic antialiasing of `color` [B,H,W,C] (any C >= 1) along silhouette edges, the stand-in for dr.antialias in render_mesh's
+    composite_buffer (render/render.py:290).  rast from `rasterize`, pos the clip-space vertices [V,4] or [B,V,4] it was made from,
+    tri int32 [T,3], topology from `antialias_topology(tri)` (built inside the call when None; pass it to share one build between
+    the buffers of a frame).  Differentiable with respect to color and pos; rast carries no gradient.  The output is a
+    deterministic per-pixel gather and antialias is linear in color for fixed geometry, so channels of several buffers may be
+    concatenated into one call.  Semantics: csrc/raster.cu."""
+    L.require_cuda(color, rast, pos, tri)
+    if color.dim() != 4 or color.shape[3] < 1:
+        raise ValueError("antialias: color must be [B,H,W,C], got %s" % (tuple(color.shape),))
+    if not color.is_floating_point() or rast.dtype != torch.float32:
+        raise TypeError("antialias: color must be floating point and rast fp32")
+    if rast.dim() != 4 or rast.shape[3] != 4 or rast.shape[:3] != color.shape[:3]:
+        raise ValueError("antialias: rast must be [B,H,W,4] matching color %s, got %s" % (tuple(color.shape), tuple(rast.shape)))
+    _check_pos(pos, color.shape[0], "antialias")
+    _check_tri(tri, "antialias")
+    if topology is None:
+        topology = antialias_topology(tri)
+    else:
+        L.require_cuda(topology)
+        _check_tri(topology, "antialias", "topology")
+        if topology.shape[0] != tri.shape[0]:
+            raise ValueError("antialias: topology has %d rows for %d triangles" % (topology.shape[0], tri.shape[0]))
+    return _antialias_func.apply(color.to(torch.float32).contiguous(), pos.contiguous(), rast.detach().contiguous(), tri.contiguous(),
+                                 topology.contiguous())
 
 
 class _texel_fetch_func(torch.autograd.Function):

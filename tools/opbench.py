@@ -30,6 +30,85 @@ def timed(fn, reps=20):
 
 out = {"hbm_peak_gbs": peak, "peak_source": peak_src, "l2_policy": "1 GB buffer rewritten between timed iterations", "ops": []}
 g = torch.Generator().manual_seed(0)
+
+
+def geometry_ops():
+    """Geometry-gradient kernels at 8 x 512 x 512, C = 4, on the bench mesh (C-ABI calls on preallocated buffers, so the times are the
+    kernels'), plus the adjacency build at 7 k and 1.08 M triangles.  Algorithmic bytes per pixel: rasterize_bwd reads rast + d_rast
+    (32 B); interpolate_bwd_rast reads rast + d_out and writes d_rast (32 + 4C B); antialias fwd reads color + rast, writes out
+    (8C + 16 B); antialias bwd reads color + d_out + rast, writes d_color (12C + 16 B); neighbour reads hit L1 / L2."""
+    from nvdiffrecmc_b200 import _lib as L
+    from nvdiffrecmc_b200 import raster
+    res = {}
+    v, f, _ = bench.build_scene_numpy(bench.WORKLOAD, 0)
+    vt, ft = torch.tensor(v, device=dev), torch.tensor(f, device=dev)
+    ctx = ou.OptiXContext()
+    ou.optix_build_bvh(ctx, vt, ft, rebuild=1)
+    B, H, W, Cc = 8, 512, 512, 4
+    mtx = torch.tensor(np.stack([synth.perspective(n=0.1, f=10.0) @ synth.orbit_view(2 * np.pi * b / B) for b in range(B)]).astype(np.float32), device=dev)
+    pos = ru.xfm_points(vt[None], mtx).detach().contiguous()
+    rast = raster.rasterize(ctx, mtx, (H, W))
+    V, T, npx = pos.shape[1], ft.shape[0], B * H * W
+    ids = rast[..., 3]
+    disc = torch.zeros_like(ids, dtype=torch.bool)
+    disc[:, :, 1:] |= ids[:, :, 1:] != ids[:, :, :-1]; disc[:, :, :-1] |= ids[:, :, 1:] != ids[:, :, :-1]
+    disc[:, 1:] |= ids[:, 1:] != ids[:, :-1]; disc[:, :-1] |= ids[:, 1:] != ids[:, :-1]
+    res["shape"] = [B, H, W, Cc]; res["triangles"] = T
+    res["covered_px_frac"] = round(float((ids > 0).float().mean()), 4); res["px_with_a_discontinuity_frac"] = round(float(disc.float().mean()), 4)
+    d_rast = torch.randn(B, H, W, 4, generator=g).to(dev)
+    d_pos = torch.zeros_like(pos)
+    lib, st = L.lib(), L.stream_ptr()
+
+    def rbwd():
+        d_pos.zero_()
+        lib.mcs_rasterize_bwd(pos.data_ptr(), V * 4, V, ft.data_ptr(), T, rast.data_ptr(), B, H, W, d_rast.data_ptr(), d_pos.data_ptr(), st)
+    ms = timed(rbwd)
+    res["rasterize_bwd"] = {"ms": round(ms, 4), "gbs_at_32B_per_px": round(npx * 32 / ms / 1e6, 1), "covered_px": int((ids > 0).sum())}
+    attr = torch.rand(V, Cc, generator=g).to(dev)
+    d_out = torch.randn(B, H, W, Cc, generator=g).to(dev)
+    d_attr = torch.zeros_like(attr); d_r = torch.empty_like(rast)
+    for name, da in (("interpolate_bwd_rast", d_attr), ("interpolate_bwd_rast_no_attr_grad", None)):
+        ms = timed(lambda: lib.mcs_interpolate_bwd_rast(attr.data_ptr(), 0, V, Cc, ft.data_ptr(), T, rast.data_ptr(), B, H, W, d_out.data_ptr(),
+                                                        da.data_ptr() if da is not None else None, d_r.data_ptr(), st))
+        res[name] = {"ms": round(ms, 4), "gbs_at_%dB_per_px" % (32 + 4 * Cc): round(npx * (32 + 4 * Cc) / ms / 1e6, 1)}
+    topo = raster.antialias_topology(ft)
+    color = torch.rand(B, H, W, Cc, generator=g).to(dev)
+    out_c = torch.empty_like(color); d_c = torch.empty_like(color)
+    aa = (color.data_ptr(), Cc, rast.data_ptr(), B, H, W, pos.data_ptr(), V * 4, V, ft.data_ptr(), T, topo.data_ptr())
+    ms_f = timed(lambda: lib.mcs_antialias_fwd(*aa, out_c.data_ptr(), st))
+
+    def aab():
+        d_pos.zero_()
+        lib.mcs_antialias_bwd(*aa, d_out.data_ptr(), d_c.data_ptr(), d_pos.data_ptr(), st)
+    ms_b = timed(aab)
+    fb, bb = 8 * Cc + 16, 12 * Cc + 16
+    res["antialias"] = {"fwd_ms": round(ms_f, 4), "fwd_gbs_at_%dB_per_px" % fb: round(npx * fb / ms_f / 1e6, 1),
+                        "fwd_frac_of_hbm_peak": round(npx * fb / ms_f / 1e6 / peak, 3), "bwd_ms": round(ms_b, 4),
+                        "bwd_gbs_at_%dB_per_px" % bb: round(npx * bb / ms_b / 1e6, 1), "bwd_frac_of_hbm_peak": round(npx * bb / ms_b / 1e6 / peak, 3)}
+    ws = torch.empty(int(lib.mcs_aa_topology_workspace_bytes(T)), dtype=torch.uint8, device=dev)
+    res["aa_topology"] = []
+    for kind in ("blob+torus", "grid1m"):
+        if kind == "grid1m":
+            v1, f1 = synth.scene_mesh("grid1m")
+            ftk = torch.tensor(f1, device=dev)
+            ws = torch.empty(int(lib.mcs_aa_topology_workspace_bytes(ftk.shape[0])), dtype=torch.uint8, device=dev)
+        else:
+            ftk = ft
+        adj = torch.empty_like(ftk)
+        ms = timed(lambda: lib.mcs_aa_topology(ftk.data_ptr(), ftk.shape[0], ws.data_ptr(), adj.data_ptr(), st))
+        res["aa_topology"].append({"mesh": kind, "triangles": int(ftk.shape[0]), "ms": round(ms, 4), "workspace_mb": round(ws.numel() / 1e6, 1),
+                                   "mtris_per_s": round(ftk.shape[0] / ms / 1e3, 1)})
+    return res
+
+
+if os.environ.get("OPB_ONLY") in (None, "geo"):
+    out["geometry"] = geometry_ops()
+    print(out["geometry"], flush=True)
+    if os.environ.get("OPB_ONLY") == "geo":
+        if len(sys.argv) > 1:
+            json.dump(out, open(sys.argv[1], "w"), indent=1)
+        sys.exit(0)
+
 for shape in [(1, 256, 256), (16, 512, 512), (1, 2048, 2048)]:          # test_bsdf.py RES-like + test_perf.py:54-56 sizes
     B, H, W = shape
     npx = B * H * W

@@ -47,6 +47,14 @@ a4 = (torch.rand(2, 12, 12, 4, device=dev) + 0.5).requires_grad_(True)
 shade_combine(a4, a4 * 1.5, t("kd"), t("ks")).sum().backward()
 tex = torch.rand(64, 3, device=dev, requires_grad=True)
 texel_fetch(tex, torch.randint(0, 64, (2, 12, 12), device=dev)).sum().backward()
+# geometry gradients: rasterize backward, interpolate backward to rast (no attribute gradient), edge adjacency, antialias fwd / bwd
+from nvdiffrecmc_b200.raster import rasterize, interpolate, antialias, antialias_topology
+mg = (proj @ mv)[None]
+posg = ru.xfm_points(t("verts")[None], mg).detach().requires_grad_(True)
+rg = rasterize(ctx, mg, (24, 24), pos=posg, tri=t("tris"))
+ig, _ = interpolate(t("verts"), rg, t("tris"))
+antialias(torch.cat([ig, rg[..., 3:4].clamp(0, 1)], -1), rg, posg, t("tris")).sum().backward()
+antialias(torch.rand(1, 24, 24, 1, device=dev), rg.detach(), posg.detach()[0], t("tris"), antialias_topology(t("tris")))
 if os.environ.get("MCS_EW_TMA"):
     B, H, W = 1, 400, 400          # 160 000 px = 312 tiles of 512 px (>= 2 x 132) + a ragged tail
     ins = [torch.rand(B, H, W, 3, device=dev).requires_grad_(True) for _ in range(6)]

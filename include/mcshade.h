@@ -53,6 +53,11 @@ int mcs_bvh_build(mcs_ctx *ctx, const float *verts, int32_t V, const int32_t *tr
  * T, T, T-1, T-1, (2T-1)*3, (2T-1)*3.  Node ids: internal 0..T-2, leaf j = T-1+j. */
 int mcs_bvh_export(mcs_ctx *ctx, uint32_t *morton, int32_t *prim, int32_t *left, int32_t *right, float *lo, float *hi, mcs_stream stream);
 
+/* Test / inspection hook: copies the shadow-ray view that env_shade walks into caller-provided DEVICE
+ * buffers: the 4-wide quantised nodes (max(T-1,1) x 4 x uint4), the triangle records its leaf runs
+ * index (T x 3 float4: (v0, original id), (e1, -), (e2, -)) and the grid (origin, cell, 1 / cell). */
+int mcs_bvh_export_shadow(mcs_ctx *ctx, uint32_t *nodesq4, float *tris, float *qgrid, mcs_stream stream);
+
 /* Any-hit visibility of n rays (origin, direction; t in (0, 1e16)), the "integer visibility mask":
  * vis[i] = 1 if nothing is hit.  Same predicate as the shadow rays inside env_shade; replaces
  * shadow_test()/optixTrace, optixutils/c_src/envsampling/kernel.cu:101-118. */

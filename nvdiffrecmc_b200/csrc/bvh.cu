@@ -3,7 +3,7 @@
 // Replaces optix_build_bvh -> optixAccelBuild (render/optixutils/c_src/torch_bindings.cpp:37-116),
 // which the training loop calls EVERY iteration (geometry/dlmesh.py:50, dmtet.py:202).  The
 // reference cudaFree/cudaMalloc's its buffers per call and builds on legacy stream 0; here the
-// whole build is 11 hand-written launches on the caller's stream (incl. the onesweep radix sort), no host sync, no
+// whole build is 11 hand-written launches (13 with the shadow view's own topology) on the caller's stream (incl. the onesweep radix sort), no host sync, no
 // allocation in steady state (ctx.h), no library code.
 //
 // Pipeline (canonical, bit-identical to oracle/mcoracle.c:orc_lbvh_build so the integer structure
@@ -17,7 +17,9 @@
 //                    box union with arrival counters (second thread to arrive continues)
 //   6. emit        : 64-byte fp32 binary traversal nodes holding both children's boxes (stand-alone visibility / closest-hit queries)
 //   7. emit_nodesq : 16-bit quantised child records on a scene-wide power-of-two grid, as a 4-wide (4 x 16 B: the grandchildren
-//                    of binary node i) view of the same tree -- what the fused kernel's shadow rays walk
+//                    of binary node i) view of the same tree -- what the fused kernel's shadow rays walk above MCS_SAH_MAX_TRIS
+//   8. ploc + emit_shadow (5 <= T <= MCS_SAH_MAX_TRIS, two more launches): the shadow rays' 4-wide view gets its own SAH
+//                    topology and its own triangle order instead (see k_ploc)
 #include "bvh_traverse.cuh"
 #include "ctx.h"
 
@@ -392,6 +394,40 @@ __device__ __forceinline__ void emit_node(int i, int T, const int32_t *left, con
     nodes[4 * (size_t)i + 3] = make_float4(__int_as_float(child_code(c0, T, range)), __int_as_float(child_code(c1, T, range)), 0.0f, 0.0f);
 }
 
+// Scene-wide quantisation grid of the shadow-ray view (see emit_nodeq): origin = root box min, cell = smallest power of two with
+// 65532 cells covering the root extent.  lo / hi of node 0 are the root box (for T == 1: the only leaf).
+__device__ __forceinline__ void quant_grid(const float *lo, const float *hi, float org[3], float inv_cell[3], float cell[3])
+{
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        org[a] = lo[a];
+        const float ext = __fsub_rn(hi[a], lo[a]);
+        // smallest power of two >= ext / 65532 (exponent arithmetic: no rounding in the grid itself)
+        int e;
+        const float m = frexpf(fmaxf(ext, 1e-30f) * (1.0f / 65532.0f), &e);  // value = m * 2^e, m in [0.5, 1)
+        const int k = (m == 0.5f) ? e - 1 : e;
+        inv_cell[a] = ldexpf(1.0f, -k);
+        cell[a] = ldexpf(1.0f, k);
+    }
+}
+
+// One 16-byte child record: the box rounded outward on the grid and inflated by two cells per side; l == nullptr is an unused slot
+// (inverted box, never entered).
+__device__ __forceinline__ uint4 quant_child(const float *l, const float *h, const float org[3], const float inv_cell[3], uint32_t word)
+{
+    uint32_t ql[3] = {65535u, 65535u, 65535u}, qh[3] = {0u, 0u, 0u};
+    if (l) {
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            const float fl = floorf(__fmul_rn(__fsub_rn(l[a], org[a]), inv_cell[a])) - 2.0f;
+            const float fh = ceilf(__fmul_rn(__fsub_rn(h[a], org[a]), inv_cell[a])) + 2.0f;
+            ql[a] = (uint32_t)fminf(fmaxf(fl, 0.0f), 65535.0f);
+            qh[a] = (uint32_t)fminf(fmaxf(fh, 0.0f), 65535.0f);
+        }
+    }
+    return make_uint4(ql[0] | (qh[0] << 16), ql[1] | (qh[1] << 16), ql[2] | (qh[2] << 16), word);
+}
+
 // Quantised 4-wide view of the tree for the shadow rays.  The fused kernel's trace loop is instruction-issue bound; with fp32
 // 64-byte binary nodes (four loads per visit) the L1 data pipe was a co-limiter as well (75 % busy, profiles/r01_v5_*).  A child
 // record with its box as 16-bit integers on ONE scene-wide grid is 16 bytes -- one 128-bit load per child:
@@ -405,20 +441,12 @@ __device__ __forceinline__ void emit_node(int i, int T, const int32_t *left, con
 __device__ __forceinline__ void emit_nodeq(const int i, int T, const int32_t *left, const int32_t *right, const int2 *range, const float *lo, const float *hi,
                                            uint4 *nodesq4, float *qgrid)
 {
-    float org[3], inv_cell[3];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        org[a] = lo[a];                                                      // node 0 = root (for T == 1: the only leaf)
-        const float ext = __fsub_rn(hi[a], lo[a]);
-        // smallest power of two >= ext / 65532 (exponent arithmetic: no rounding in the grid itself)
-        int e;
-        const float m = frexpf(fmaxf(ext, 1e-30f) * (1.0f / 65532.0f), &e);  // value = m * 2^e, m in [0.5, 1)
-        const int k = (m == 0.5f) ? e - 1 : e;
-        inv_cell[a] = ldexpf(1.0f, -k);
-        if (i == 0) { qgrid[a] = org[a]; qgrid[3 + a] = ldexpf(1.0f, k); qgrid[6 + a] = inv_cell[a]; }
-    }
+    float org[3], inv_cell[3], cell[3];
+    quant_grid(lo, hi, org, inv_cell, cell);
+    if (i == 0)
+        for (int a = 0; a < 3; ++a) { qgrid[a] = org[a]; qgrid[3 + a] = cell[a]; qgrid[6 + a] = inv_cell[a]; }
     const bool tiny = T <= MCS_LEAF_MAX;
-    if (tiny ? i != 0 : i >= T - 1) return;
+    if (!nodesq4 || (tiny ? i != 0 : i >= T - 1)) return;
     int cn[2], code[2];
     if (tiny) { cn[0] = 0; cn[1] = -1; code[0] = ~((0 << 3) | (T - 1)); code[1] = ~0; }
     else { cn[0] = left[i]; cn[1] = right[i]; code[0] = child_code(cn[0], T, range); code[1] = child_code(cn[1], T, range); }
@@ -445,28 +473,219 @@ __device__ __forceinline__ void emit_nodeq(const int i, int T, const int32_t *le
     for (int c = 0; c < 4; ++c) leaf_bits |= (gcode[c] < 0 ? 1u : 0u) << c;
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-        uint32_t ql[3] = {65535u, 65535u, 65535u}, qh[3] = {0u, 0u, 0u};
-        if (gn[c] >= 0) {
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                const float fl = floorf(__fmul_rn(__fsub_rn(lo[3 * (size_t)gn[c] + a], org[a]), inv_cell[a])) - 2.0f;
-                const float fh = ceilf(__fmul_rn(__fsub_rn(hi[3 * (size_t)gn[c] + a], org[a]), inv_cell[a])) + 2.0f;
-                ql[a] = (uint32_t)fminf(fmaxf(fl, 0.0f), 65535.0f);
-                qh[a] = (uint32_t)fminf(fmaxf(fh, 0.0f), 65535.0f);
-            }
-        }
         const uint32_t payload = (uint32_t)(gcode[c] < 0 ? ~gcode[c] : gcode[c]) & 0x0FFFFFFFu;
-        nodesq4[4 * (size_t)i + c] = make_uint4(ql[0] | (qh[0] << 16), ql[1] | (qh[1] << 16), ql[2] | (qh[2] << 16), payload | (c == 0 ? leaf_bits << 28 : 0u));
+        const bool used = gn[c] >= 0;
+        nodesq4[4 * (size_t)i + c] = quant_child(used ? lo + 3 * (size_t)gn[c] : nullptr, used ? hi + 3 * (size_t)gn[c] : nullptr, org, inv_cell,
+                                                 payload | (c == 0 ? leaf_bits << 28 : 0u));
     }
 }
 
-// one launch for both node views (large-mesh path)
+// One launch for both node views.  nodesq4 == nullptr: only the grid is written (the shadow-ray view comes from k_emit_shadow).
 __global__ void __launch_bounds__(256) k_emit_both(int T, const int32_t *left, const int32_t *right, const int2 *range, const float *lo, const float *hi,
                                                    float4 *nodes, uint4 *nodesq4, float *qgrid)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     emit_node(i, T, left, right, range, lo, hi, nodes);
     emit_nodeq(i, T, left, right, range, lo, hi, nodesq4, qgrid);
+}
+
+// ---------------------------------------------------------------------------------------------
+// SAH topology for the shadow-ray view.  The any-hit shadow rays (two env_shade launches per training step) are most of the
+// step; the Morton LBVH they used to walk is the lowest-quality tree in common use.  So the shadow view gets its own tree, rebuilt
+// with the LBVH every iteration (the geometry is trainable):
+//   * k_ploc: PLOC clustering (Meister & Bittner, "Parallel Locally-Ordered Clustering for BVH construction", TVCG 2018) over the
+//     leaves in Morton order, in ONE CTA: every cluster finds its nearest neighbour (smallest merged surface area) among the
+//     PLOC_RADIUS clusters on either side, mutual pairs merge, the array is compacted in order; repeat until one cluster is left.
+//     Ties go to the lower index, so the minimum-area pair of every round is mutual and each round merges at least one pair.  A
+//     merged node is collapsed to a leaf run when it has <= SAH_LEAF_MAX triangles and the leaf's SAH cost does not exceed the
+//     subtree's.  Then, top-down in reverse creation order, every node gets the first slot of its triangles in depth-first
+//     leaf order, so the triangles of every subtree (and of every leaf run) are consecutive.
+//   * k_emit_shadow: the triangle records in that order, and the 4-wide quantised nodes by an SAH-greedy collapse (open the
+//     internal child of largest surface area until there are four).  Record format, leaf nibble, grid and inflation as emit_nodeq.
+// The canonical LBVH, its fp32 nodes and its Morton-ordered triangle records (closest-hit queries, trace_visibility, export) are
+// not touched.  Above MCS_SAH_MAX_TRIS triangles one CTA takes too long and the shadow view stays the LBVH grandchild collapse.
+// A refit (rebuild = 0) reruns the clustering on the refitted leaf boxes in the Morton order of the last rebuild.
+// ---------------------------------------------------------------------------------------------
+#ifndef MCS_SAH_MAX_TRIS
+#define MCS_SAH_MAX_TRIS 16384
+#endif
+#define PLOC_THREADS 1024
+#define PLOC_RADIUS 8           // radius 16: same kernel time on the bench mesh, 130 us more per rebuild
+#define SAH_LEAF_MAX 8          // 3-bit count field of a leaf run
+#define SAH_CI 1.2f             // cost of a binary node relative to one triangle test (2.0: equal, 3.0: slower kernel)
+#define SAH_CT 1.0f
+
+__device__ __forceinline__ float half_area(float4 l, float4 h)
+{
+    const float dx = h.x - l.x, dy = h.y - l.y, dz = h.z - l.z;
+    return dx * dy + dy * dz + dz * dx;
+}
+
+// exclusive block scan of two counters (PLOC_THREADS threads); *total = the sums
+__device__ __forceinline__ int2 block_exscan2(int2 v, int2 *total, int2 *sw)
+{
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int2 x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int yx = __shfl_up_sync(0xFFFFFFFFu, x.x, o), yy = __shfl_up_sync(0xFFFFFFFFu, x.y, o);
+        if (lane >= o) { x.x += yx; x.y += yy; }
+    }
+    if (lane == 31) sw[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        int2 w = sw[lane];
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int yx = __shfl_up_sync(0xFFFFFFFFu, w.x, o), yy = __shfl_up_sync(0xFFFFFFFFu, w.y, o);
+            if (lane >= o) { w.x += yx; w.y += yy; }
+        }
+        sw[lane] = w;
+    }
+    __syncthreads();
+    const int2 base = warp ? sw[warp - 1] : make_int2(0, 0);
+    *total = sw[31];
+    return make_int2(base.x + x.x - v.x, base.y + x.y - v.y);
+}
+
+struct ShadowTree {
+    int32_t *left, *right;  // [T-1] children (internal 0..T-2, root 0; leaf of sorted triangle j: T-1+j)
+    float4 *box;            // [T-1][2] lo (w: unused), hi
+    int32_t *cnt;           // [T-1] triangles under the node; negative: the node is a leaf run of -cnt triangles
+    int32_t *first;         // [2T-1] first slot of the node's triangles in depth-first leaf order
+};
+
+// Scratch: cluster ids [2][T], cluster boxes [2][T][2] (lo.w = SAH cost, hi.w = triangle count), nearest neighbour [T], next free
+// node id before each round [T].
+__global__ void __launch_bounds__(PLOC_THREADS) k_ploc(int T, const float *lo, const float *hi, ShadowTree st, int32_t *cid, float4 *cbox, int32_t *nn,
+                                                       int32_t *round_id)
+{
+    __shared__ int2 sw[32];
+    const int tid = threadIdx.x;
+    for (int j = tid; j < T; j += PLOC_THREADS) {
+        const size_t n = (size_t)(T - 1 + j);
+        const float4 l = make_float4(lo[3 * n], lo[3 * n + 1], lo[3 * n + 2], 0.0f), h = make_float4(hi[3 * n], hi[3 * n + 1], hi[3 * n + 2], 0.0f);
+        cid[j] = T - 1 + j;
+        cbox[2 * j] = make_float4(l.x, l.y, l.z, SAH_CT * half_area(l, h));
+        cbox[2 * j + 1] = make_float4(h.x, h.y, h.z, __int_as_float(1));
+    }
+    __syncthreads();
+    int n = T, next_id = T - 2, rounds = 0, buf = 0;
+    while (n > 1) {
+        int32_t *ci = cid + (size_t)buf * T, *co = cid + (size_t)(buf ^ 1) * T;
+        float4 *bi = cbox + (size_t)buf * 2 * T, *bo = cbox + (size_t)(buf ^ 1) * 2 * T;
+        if (tid == 0) round_id[rounds] = next_id;
+        // ---- nearest neighbour within the radius (ties: lower index) ----
+        for (int i = tid; i < n; i += PLOC_THREADS) {
+            const float4 li = bi[2 * i], hi_ = bi[2 * i + 1];
+            float best = INFINITY;
+            int bj = -1;
+            const int j0 = max(0, i - PLOC_RADIUS), j1 = min(n - 1, i + PLOC_RADIUS);
+            for (int j = j0; j <= j1; ++j) {
+                if (j == i) continue;
+                const float4 lj = bi[2 * j], hj = bi[2 * j + 1];
+                // (NaN -> +inf keeps the order total, so a mutual pair exists even for non-finite geometry)
+                const float a = fminf(half_area(make_float4(fminf(li.x, lj.x), fminf(li.y, lj.y), fminf(li.z, lj.z), 0.0f),
+                                                make_float4(fmaxf(hi_.x, hj.x), fmaxf(hi_.y, hj.y), fmaxf(hi_.z, hj.z), 0.0f)), INFINITY);
+                if (a < best || bj < 0) { best = a; bj = j; }
+            }
+            nn[i] = bj;
+        }
+        __syncthreads();
+        // ---- merge mutual pairs (the lower index keeps the merged cluster), compact in order ----
+        const int per = (n + PLOC_THREADS - 1) / PLOC_THREADS, beg = min(n, tid * per), end = min(n, beg + per);
+        int2 mine = make_int2(0, 0);            // (clusters kept, merges)
+        for (int i = beg; i < end; ++i) {
+            const int j = nn[i];
+            const bool mutual = nn[j] == i;
+            mine.x += (!mutual || i < j) ? 1 : 0;
+            mine.y += (mutual && i < j) ? 1 : 0;
+        }
+        int2 tot;
+        int2 pos = block_exscan2(mine, &tot, sw);
+        for (int i = beg; i < end; ++i) {
+            const int j = nn[i];
+            const bool mutual = nn[j] == i;
+            if (mutual && i > j) continue;
+            if (!mutual) { co[pos.x] = ci[i]; bo[2 * pos.x] = bi[2 * i]; bo[2 * pos.x + 1] = bi[2 * i + 1]; ++pos.x; continue; }
+            const float4 la = bi[2 * i], ha = bi[2 * i + 1], lb = bi[2 * j], hb = bi[2 * j + 1];
+            const float4 l = make_float4(fminf(la.x, lb.x), fminf(la.y, lb.y), fminf(la.z, lb.z), 0.0f);
+            const float4 h = make_float4(fmaxf(ha.x, hb.x), fmaxf(ha.y, hb.y), fmaxf(ha.z, hb.z), 0.0f);
+            const float A = half_area(l, h);
+            const int cnt = __float_as_int(ha.w) + __float_as_int(hb.w);
+            const float c_int = SAH_CI * A + la.w + lb.w, c_leaf = SAH_CT * A * (float)cnt;
+            const bool leaf = cnt <= SAH_LEAF_MAX && c_leaf <= c_int;
+            const int id = next_id - pos.y;
+            st.left[id] = ci[i]; st.right[id] = ci[j];
+            st.box[2 * id] = l; st.box[2 * id + 1] = h;
+            st.cnt[id] = leaf ? -cnt : cnt;
+            co[pos.x] = id;
+            bo[2 * pos.x] = make_float4(l.x, l.y, l.z, leaf ? c_leaf : c_int);
+            bo[2 * pos.x + 1] = make_float4(h.x, h.y, h.z, __int_as_float(cnt));
+            ++pos.x; ++pos.y;
+        }
+        n = tot.x; next_id -= tot.y; buf ^= 1; ++rounds;
+        __syncthreads();
+    }
+    // ---- depth-first leaf order, top-down: a node is created in a later round than its children ----
+    if (tid == 0) { round_id[rounds] = next_id; st.first[0] = 0; }      // next_id == -1: the last merge created the root, node 0
+    __syncthreads();
+    for (int r = rounds - 1; r >= 0; --r) {
+        for (int id = round_id[r + 1] + 1 + tid; id <= round_id[r]; id += PLOC_THREADS) {
+            const int f = st.first[id], l = st.left[id];
+            st.first[l] = f;
+            st.first[st.right[id]] = f + (l >= T - 1 ? 1 : abs(st.cnt[l]));
+        }
+        __syncthreads();
+    }
+}
+
+__global__ void __launch_bounds__(256) k_emit_shadow(int T, ShadowTree st, const float *lo, const float *hi, const float4 *__restrict__ tris,
+                                                     float4 *__restrict__ stris, uint4 *__restrict__ nodesq4)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= T) return;
+    {   // triangle records in depth-first leaf order
+        const int d = st.first[T - 1 + i];
+        stris[3 * (size_t)d] = tris[3 * (size_t)i];
+        stris[3 * (size_t)d + 1] = tris[3 * (size_t)i + 1];
+        stris[3 * (size_t)d + 2] = tris[3 * (size_t)i + 2];
+    }
+    if (i >= T - 1 || (i != 0 && st.cnt[i] < 0)) return;       // leaf runs have no node (the root is always a node)
+    auto is_node = [&](int x) { return x < T - 1 && st.cnt[x] > 0; };
+    int s[4] = {st.left[i], st.right[i], -1, -1}, ns = 2;
+    while (ns < 4) {     // open the internal child of largest surface area
+        int b = -1;
+        float ba = -1.0f;
+        for (int c = 0; c < ns; ++c)
+            if (is_node(s[c])) {
+                const float a = half_area(st.box[2 * s[c]], st.box[2 * s[c] + 1]);
+                if (a > ba) { ba = a; b = c; }
+            }
+        if (b < 0) break;
+        const int x = s[b];
+        s[b] = st.left[x]; s[ns++] = st.right[x];
+    }
+    float org[3], inv_cell[3], cell[3];
+    quant_grid(lo, hi, org, inv_cell, cell);
+    uint32_t leaf_bits = 0u;
+    for (int c = 0; c < 4; ++c) leaf_bits |= (c >= ns || !is_node(s[c]) ? 1u : 0u) << c;
+    for (int c = 0; c < 4; ++c) {
+        uint32_t payload = 0u;
+        const float *l = nullptr, *h = nullptr;
+        float bl[3], bh[3];
+        if (c < ns) {
+            const int x = s[c];
+            if (x >= T - 1) { l = lo + 3 * (size_t)x; h = hi + 3 * (size_t)x; payload = (uint32_t)st.first[x] << 3; }
+            else {
+                const float4 a = st.box[2 * x], b = st.box[2 * x + 1];
+                bl[0] = a.x; bl[1] = a.y; bl[2] = a.z; bh[0] = b.x; bh[1] = b.y; bh[2] = b.z;
+                l = bl; h = bh;
+                payload = st.cnt[x] > 0 ? (uint32_t)x : ((uint32_t)st.first[x] << 3) | (uint32_t)(-st.cnt[x] - 1);
+            }
+        }
+        nodesq4[4 * (size_t)i + c] = quant_child(l, h, org, inv_cell, (payload & 0x0FFFFFFFu) | (c == 0 ? leaf_bits << 28 : 0u));
+    }
 }
 
 typedef BvhView VisView;
@@ -511,7 +730,7 @@ int mcs_ctx_destroy(mcs_ctx *c)
     if (!c) return 0;
     DevBuf *bufs[] = {&c->bounds, &c->tlo, &c->thi, &c->keys, &c->keys_alt, &c->vals, &c->vals_alt, &c->left, &c->right, &c->parent,
                       &c->lo, &c->hi, &c->flags, &c->range, &c->sort_tmp, &c->nodes, &c->tris, &c->nodesq4, &c->qgrid, &c->lcg_skip[0], &c->lcg_skip[1], &c->lcg_skip[2], &c->lcg_skip[3],
-                      &c->counters, &c->mtx_inv};
+                      &c->counters, &c->mtx_inv, &c->sleft, &c->sright, &c->scnt, &c->sbox, &c->sfirst, &c->swork, &c->stris};
     for (DevBuf *b : bufs)
         if (b->p) cudaFree(b->p);
     delete c;
@@ -570,10 +789,29 @@ int mcs_bvh_build(mcs_ctx *c, const float *verts, int32_t V, const int32_t *tris
                                                                    (const int32_t *)c->right.p, (const int32_t *)c->parent.p, (const int2 *)c->range.p,
                                                                    (float *)c->lo.p, (float *)c->hi.p, (int *)c->flags.p, (float4 *)c->tris.p);
     MCS_LAUNCH_CHECK();
+    const bool sah = T > MCS_LEAF_MAX && T <= MCS_SAH_MAX_TRIS;
     k_emit_both<<<nblk(T > 1 ? T - 1 : 1, 256), 256, 0, s>>>(T, (const int32_t *)c->left.p, (const int32_t *)c->right.p, (const int2 *)c->range.p,
-                                                              (const float *)c->lo.p, (const float *)c->hi.p, (float4 *)c->nodes.p, (uint4 *)c->nodesq4.p,
-                                                              (float *)c->qgrid.p);
+                                                              (const float *)c->lo.p, (const float *)c->hi.p, (float4 *)c->nodes.p,
+                                                              sah ? nullptr : (uint4 *)c->nodesq4.p, (float *)c->qgrid.p);
     MCS_LAUNCH_CHECK();
+    if (sah) {
+        if (int e = mcs_buf_reserve(c->sleft, nT * sizeof(int32_t), s)) return e;
+        if (int e = mcs_buf_reserve(c->sright, nT * sizeof(int32_t), s)) return e;
+        if (int e = mcs_buf_reserve(c->scnt, nT * sizeof(int32_t), s)) return e;
+        if (int e = mcs_buf_reserve(c->sbox, nT * 2 * sizeof(float4), s)) return e;
+        if (int e = mcs_buf_reserve(c->sfirst, nN * sizeof(int32_t), s)) return e;
+        if (int e = mcs_buf_reserve(c->swork, nT * (4 * sizeof(float4) + 4 * sizeof(int32_t)), s)) return e;
+        if (int e = mcs_buf_reserve(c->stris, nT * 3 * sizeof(float4), s)) return e;
+        const ShadowTree st{(int32_t *)c->sleft.p, (int32_t *)c->sright.p, (float4 *)c->sbox.p, (int32_t *)c->scnt.p, (int32_t *)c->sfirst.p};
+        float4 *cbox = (float4 *)c->swork.p;                      // [2][T][2]
+        int32_t *cid = (int32_t *)(cbox + 4 * nT);                // [2][T]
+        k_ploc<<<1, PLOC_THREADS, 0, s>>>(T, (const float *)c->lo.p, (const float *)c->hi.p, st, cid, cbox, cid + 2 * nT, cid + 3 * nT);
+        MCS_LAUNCH_CHECK();
+        k_emit_shadow<<<nblk(T, 256), 256, 0, s>>>(T, st, (const float *)c->lo.p, (const float *)c->hi.p, (const float4 *)c->tris.p, (float4 *)c->stris.p,
+                                                   (uint4 *)c->nodesq4.p);
+        MCS_LAUNCH_CHECK();
+    }
+    c->shadow_sah = sah;
     c->T = T; c->V = V;
     return 0;
 }
@@ -591,6 +829,17 @@ int mcs_bvh_export(mcs_ctx *c, uint32_t *morton, int32_t *prim, int32_t *left, i
     }
     MCS_CUDA(cudaMemcpyAsync(lo, c->lo.p, (2 * T - 1) * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     MCS_CUDA(cudaMemcpyAsync(hi, c->hi.p, (2 * T - 1) * 3 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return 0;
+}
+
+int mcs_bvh_export_shadow(mcs_ctx *c, uint32_t *nodesq4, float *tris, float *qgrid, mcs_stream stream)
+{
+    cudaStream_t s = (cudaStream_t)stream;
+    MCS_REQUIRE(c && c->T > 0, "mcs_bvh_export_shadow: no acceleration structure built");
+    const size_t T = (size_t)c->T;
+    MCS_CUDA(cudaMemcpyAsync(nodesq4, c->nodesq4.p, (T > 1 ? T - 1 : 1) * 4 * sizeof(uint4), cudaMemcpyDeviceToDevice, s));
+    MCS_CUDA(cudaMemcpyAsync(tris, c->shadow_sah ? c->stris.p : c->tris.p, T * 3 * sizeof(float4), cudaMemcpyDeviceToDevice, s));
+    MCS_CUDA(cudaMemcpyAsync(qgrid, c->qgrid.p, 9 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return 0;
 }
 

@@ -32,6 +32,13 @@ struct mcs_ctx {
     DevBuf tris;                 // [T] x 3 float4 in SORTED order: (v0, orig id), (e1, -), (e2, -)
     DevBuf nodesq4;              // [max(T-1,1)] x 4 uint4: 4-wide quantised view (the <= 4 grandchildren of binary node i), 16-bit boxes on a scene-wide grid
     DevBuf qgrid;                // 9 floats: grid origin xyz, cell size xyz, 1 / cell size xyz
+    // ---- shadow-ray view with its own SAH topology (bvh.cu:k_ploc; MCS_LEAF_MAX < T <= MCS_SAH_MAX_TRIS) ----
+    bool shadow_sah = false;     // nodesq4 walks the SAH tree and its leaf runs index stris; else the LBVH view and tris
+    DevBuf sleft, sright, scnt;  // [T-1] children, triangle counts (negative: leaf run)
+    DevBuf sbox;                 // [T-1] x 2 float4 node boxes
+    DevBuf sfirst;               // [2T-1] first slot of each node's triangles in depth-first leaf order
+    DevBuf swork;                // clustering scratch
+    DevBuf stris;                // [T] x 3 float4: the triangle records of `tris` in depth-first leaf order
     // ---- env_shade support ----
     DevBuf lcg_skip[MCS_SKIP_TABLES];   // [5*N*N+3] x uint2 (mul, add) LCG jump-ahead tables, one per cached n_samples_x
     int skip_N[MCS_SKIP_TABLES] = {0, 0, 0, 0};

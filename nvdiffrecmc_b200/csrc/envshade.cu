@@ -301,6 +301,12 @@ __device__ __forceinline__ float warp_sum(float v)
 #ifndef MCS_REFILL_BELOW
 #define MCS_REFILL_BELOW 24               // idle lanes are refilled when fewer than this many are walking (picking up a ray is cheap: rayq_fetch)
 #endif
+#ifndef MCS_COUNT_TRAVERSAL
+#define MCS_COUNT_TRAVERSAL 0             // 1: developer variant (tools/build_variant.sh) that counts rays, node visits and triangle tests
+#endif
+#if MCS_COUNT_TRAVERSAL
+__device__ unsigned long long g_trace_counts[3];   // rays fetched, 4-wide node visits, leaf-triangle tests (read by mcs_trace_counts)
+#endif
 constexpr int NW = MCS_CTA_WARPS;
 constexpr int SEG = 128;                 // queue entries per warp segment (= one pixel at N = 8)
 constexpr int QTOT = NW * SEG;
@@ -567,6 +573,9 @@ __device__ __forceinline__ void trace_queue(const EnvParams &p, BlockQueue &q, c
     const BvhView b = p.bvh;
     uint2 *pl = q.pl[warp];
     int seg = warp, exhausted = 0;           // segment being drained, number of segments found empty so far
+#if MCS_COUNT_TRAVERSAL
+    unsigned long long n_rays = 0, n_visits = 0, n_tests = 0;
+#endif
 
     auto leaf_batch = [&](int n) {
         // intersect the last n (<= 32) pending (ray, leaf run) pairs, one per lane
@@ -583,6 +592,9 @@ __device__ __forceinline__ void trace_queue(const EnvParams &p, BlockQueue &q, c
                 const f3 d = F3(q.dx[e], q.dy[e], q.dz[e]);
                 bool hit = false;
                 for (int k = 0; k < cnt && !hit; ++k) {
+#if MCS_COUNT_TRAVERSAL
+                    ++n_tests;
+#endif
                     const float4 *t = b.tris + 3 * (size_t)(start + k);
                     const float4 t0 = __ldg(t), t1 = __ldg(t + 1), t2 = __ldg(t + 2);
                     float tt, uu, vv;
@@ -612,6 +624,9 @@ __device__ __forceinline__ void trace_queue(const EnvParams &p, BlockQueue &q, c
                 my = idx;
                 r = rayq_fetch(b.qgrid, q.rog[seg], q.dx[idx], q.dy[idx], q.dz[idx]);
                 node = 0; sp = 0; sb = 0;
+#if MCS_COUNT_TRAVERSAL
+                ++n_rays;
+#endif
             }
             if (take < need) { seg = seg + 1 == NW ? 0 : seg + 1; ++exhausted; }
             idle = __ballot_sync(0xFFFFFFFFu, my < 0);
@@ -654,6 +669,9 @@ __device__ __forceinline__ void trace_queue(const EnvParams &p, BlockQueue &q, c
             unsigned lmask = 0u;
             int c0 = 0, c1 = 0, c2 = 0, c3 = 0;
             if (my >= 0) {
+#if MCS_COUNT_TRAVERSAL
+                ++n_visits;
+#endif
                 const uint4 *n = b.nodesq4 + 4 * (size_t)node;
                 const uint4 k0 = __ldg(n), k1 = __ldg(n + 1), k2 = __ldg(n + 2), k3 = __ldg(n + 3);
                 const bool h0 = qslab(k0, r), h1 = qslab(k1, r), h2 = qslab(k2, r), h3 = qslab(k3, r);
@@ -691,6 +709,9 @@ __device__ __forceinline__ void trace_queue(const EnvParams &p, BlockQueue &q, c
         // poll here instead of once per node step
         if (my >= 0 && (q.tex[my] >> 31)) my = -1;
     }
+#if MCS_COUNT_TRAVERSAL
+    atomicAdd(&g_trace_counts[0], n_rays); atomicAdd(&g_trace_counts[1], n_visits); atomicAdd(&g_trace_counts[2], n_tests);
+#endif
     __syncwarp();
 }
 
@@ -1088,7 +1109,8 @@ static int fill_params(mcs_ctx *ctx, EnvParams &p,
     p.perms = (const int32_t *)perms->ptr; p.pm_s1 = perms->strides[1]; p.pm_s3 = perms->strides[3]; p.n_perms = (uint32_t)perms->sizes[1];
     p.m_rows = cdf_iters(p.Hl); p.m_cols = cdf_iters(p.Wl);
     p.bsdf = bsdf; p.seed = rnd_seed; p.seed_dev = seed_offset_dev; p.batch_offset = batch_offset; p.shadow_scale = shadow_scale;
-    p.bvh = BvhView{(const float4 *)ctx->nodes.p, (const float4 *)ctx->tris.p, (const float *)ctx->qgrid.p, (const uint4 *)ctx->nodesq4.p};
+    p.bvh = BvhView{(const float4 *)ctx->nodes.p, (const float4 *)(ctx->shadow_sah ? ctx->stris.p : ctx->tris.p), (const float *)ctx->qgrid.p,
+                    (const uint4 *)ctx->nodesq4.p};
     if (int e = ensure_skip_table(ctx, p.N, s, &p.skip)) return e;
     // work-claim counter of the persistent grid: one slot of a small ring PER LAUNCH, so launches of the same context that are in
     // flight on different streams never share a counter
@@ -1224,5 +1246,19 @@ int mcs_env_shade_bwd_replay(const mcs_tensor *gb_pos, const mcs_tensor *gb_norm
     MCS_LAUNCH_CHECK();
     return 0;
 }
+
+#if MCS_COUNT_TRAVERSAL
+// Counting variant only (not in mcshade.h): out = {rays, node visits, triangle tests} summed over every trace since the last reset.
+int mcs_trace_counts(unsigned long long *out, int reset)
+{
+    MCS_CUDA(cudaDeviceSynchronize());
+    MCS_CUDA(cudaMemcpyFromSymbol(out, g_trace_counts, sizeof(g_trace_counts)));
+    if (reset) {
+        const unsigned long long zero[3] = {0, 0, 0};
+        MCS_CUDA(cudaMemcpyToSymbol(g_trace_counts, zero, sizeof(zero)));
+    }
+    return 0;
+}
+#endif
 
 }  // extern "C"

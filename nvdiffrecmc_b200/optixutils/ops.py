@@ -268,6 +268,18 @@ def bvh_export(optix_ctx):
     return dict(morton=morton, prim=prim, left=left[:T - 1], right=right[:T - 1], lo=lo, hi=hi)
 
 
+def bvh_export_shadow(optix_ctx):
+    """The shadow-ray view env_shade walks: 4-wide quantised nodes [max(T-1,1), 4, 4] uint32 (as int32), the triangle records its
+    leaf runs index [T, 3, 4] fp32 (original triangle id in [:, 0, 3] as int32 bits) and the grid (origin, cell, 1 / cell)."""
+    T = optix_ctx._geom[1].shape[0]
+    dev = optix_ctx._geom[0].device
+    nodes = torch.empty(max(T - 1, 1), 4, 4, dtype=torch.int32, device=dev)
+    tris = torch.empty(T, 3, 4, dtype=torch.float32, device=dev)
+    qgrid = torch.empty(9, dtype=torch.float32, device=dev)
+    L.check(L.lib().mcs_bvh_export_shadow(optix_ctx.cpp_wrapper, nodes.data_ptr(), tris.data_ptr(), qgrid.data_ptr(), L.stream_ptr()), "bvh_export_shadow")
+    return dict(nodes=nodes, tris=tris, qgrid=qgrid)
+
+
 # ----------------------------------------------------------------------------------------------
 # Bilateral denoiser (ops.py:107-119, 139-141)
 # ----------------------------------------------------------------------------------------------

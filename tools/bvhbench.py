@@ -1,4 +1,5 @@
-"""Developer tool: LBVH rebuild timing (CUDA events, L2 flushed) at the bench mesh (7 k triangles) and the 1.08 M-triangle grid;
+"""Developer tool: rebuild / refit timing (CUDA events, L2 flushed) at the bench mesh (7 k triangles) and the 1.08 M-triangle grid --
+the whole mcs_bvh_build, so up to 16 384 triangles it includes the shadow view's clustering (k_ploc, k_emit_shadow);
 run under `ncu --metrics gpu__time_duration.sum` for the per-kernel split.  usage: python tools/bvhbench.py [reps]"""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

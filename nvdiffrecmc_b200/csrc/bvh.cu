@@ -727,12 +727,6 @@ int mcs_ctx_create(mcs_ctx **out)
 
 int mcs_ctx_destroy(mcs_ctx *c)
 {
-    if (!c) return 0;
-    DevBuf *bufs[] = {&c->bounds, &c->tlo, &c->thi, &c->keys, &c->keys_alt, &c->vals, &c->vals_alt, &c->left, &c->right, &c->parent,
-                      &c->lo, &c->hi, &c->flags, &c->range, &c->sort_tmp, &c->nodes, &c->tris, &c->nodesq4, &c->qgrid, &c->lcg_skip[0], &c->lcg_skip[1], &c->lcg_skip[2], &c->lcg_skip[3],
-                      &c->counters, &c->mtx_inv, &c->sleft, &c->sright, &c->scnt, &c->sbox, &c->sfirst, &c->swork, &c->stris};
-    for (DevBuf *b : bufs)
-        if (b->p) cudaFree(b->p);
     delete c;
     return 0;
 }
@@ -746,25 +740,22 @@ int mcs_bvh_build(mcs_ctx *c, const float *verts, int32_t V, const int32_t *tris
     MCS_REQUIRE(T > 0 && V > 0, "Got empty training triangle mesh (unrecoverable discontinuity)");
     MCS_REQUIRE(T <= (1 << 25), "mcs_bvh_build: at most 2^25 triangles (28-bit child words of the quantised nodes), got %d", T);
     MCS_REQUIRE(rebuild != 0 || c->T == T, "mcs_bvh_build: refit (rebuild=0) needs an existing structure with the same triangle count (have %d, got %d)", c->T, T);
+    const bool sah = T > MCS_LEAF_MAX && T <= MCS_SAH_MAX_TRIS;       // does the shadow view get its own SAH topology?
     const size_t nT = (size_t)T, nN = 2 * nT - 1;
-    if (int e = mcs_buf_reserve(c->bounds, 12 * sizeof(uint32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->tlo, nT * 3 * sizeof(float), s)) return e;
-    if (int e = mcs_buf_reserve(c->thi, nT * 3 * sizeof(float), s)) return e;
-    if (int e = mcs_buf_reserve(c->keys, nT * sizeof(uint32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->keys_alt, nT * sizeof(uint32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->vals, nT * sizeof(int32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->vals_alt, nT * sizeof(int32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->left, nT * sizeof(int32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->right, nT * sizeof(int32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->parent, nN * sizeof(int32_t), s)) return e;
-    if (int e = mcs_buf_reserve(c->lo, nN * 3 * sizeof(float), s)) return e;
-    if (int e = mcs_buf_reserve(c->hi, nN * 3 * sizeof(float), s)) return e;
-    if (int e = mcs_buf_reserve(c->flags, nT * sizeof(int), s)) return e;
-    if (int e = mcs_buf_reserve(c->range, nT * sizeof(int2), s)) return e;
-    if (int e = mcs_buf_reserve(c->nodes, nT * 4 * sizeof(float4), s)) return e;
-    if (int e = mcs_buf_reserve(c->tris, nT * 3 * sizeof(float4), s)) return e;
-    if (int e = mcs_buf_reserve(c->nodesq4, nT * 4 * sizeof(uint4), s)) return e;
-    if (int e = mcs_buf_reserve(c->qgrid, 16 * sizeof(float), s)) return e;
+    const size_t sT = sah ? nT : 0, sN = sah ? nN : 0;                 // 0: the SAH topology's buffers are left as they are
+    const struct { DevBuf &b; size_t bytes; } need[] = {
+        {c->bounds, 12 * sizeof(uint32_t)}, {c->tlo, nT * 3 * sizeof(float)}, {c->thi, nT * 3 * sizeof(float)},
+        {c->keys, nT * sizeof(uint32_t)}, {c->keys_alt, nT * sizeof(uint32_t)}, {c->vals, nT * sizeof(int32_t)}, {c->vals_alt, nT * sizeof(int32_t)},
+        {c->left, nT * sizeof(int32_t)}, {c->right, nT * sizeof(int32_t)}, {c->parent, nN * sizeof(int32_t)},
+        {c->lo, nN * 3 * sizeof(float)}, {c->hi, nN * 3 * sizeof(float)}, {c->flags, nT * sizeof(int)}, {c->range, nT * sizeof(int2)},
+        {c->nodes, nT * 4 * sizeof(float4)}, {c->tris, nT * 3 * sizeof(float4)}, {c->nodesq4, nT * 4 * sizeof(uint4)}, {c->qgrid, 16 * sizeof(float)},
+        {c->sleft, sT * sizeof(int32_t)}, {c->sright, sT * sizeof(int32_t)}, {c->scnt, sT * sizeof(int32_t)}, {c->sbox, sT * 2 * sizeof(float4)},
+        {c->sfirst, sN * sizeof(int32_t)}, {c->cbox, sT * 4 * sizeof(float4)}, {c->cid, sT * 2 * sizeof(int32_t)}, {c->nn, sT * sizeof(int32_t)},
+        {c->round_id, sT * sizeof(int32_t)}, {c->stris, sT * 3 * sizeof(float4)},
+    };
+    for (const auto &r : need)
+        if (int e = mcs_buf_reserve(r.b, r.bytes, s)) return e;
+    c->shadow = BvhView{nullptr, (const float4 *)(sah ? c->stris.p : c->tris.p), (const float *)c->qgrid.p, (const uint4 *)c->nodesq4.p};
 
     uint32_t *bounds = (uint32_t *)c->bounds.p;
     float *tlo = (float *)c->tlo.p, *thi = (float *)c->thi.p;
@@ -789,29 +780,19 @@ int mcs_bvh_build(mcs_ctx *c, const float *verts, int32_t V, const int32_t *tris
                                                                    (const int32_t *)c->right.p, (const int32_t *)c->parent.p, (const int2 *)c->range.p,
                                                                    (float *)c->lo.p, (float *)c->hi.p, (int *)c->flags.p, (float4 *)c->tris.p);
     MCS_LAUNCH_CHECK();
-    const bool sah = T > MCS_LEAF_MAX && T <= MCS_SAH_MAX_TRIS;
     k_emit_both<<<nblk(T > 1 ? T - 1 : 1, 256), 256, 0, s>>>(T, (const int32_t *)c->left.p, (const int32_t *)c->right.p, (const int2 *)c->range.p,
                                                               (const float *)c->lo.p, (const float *)c->hi.p, (float4 *)c->nodes.p,
                                                               sah ? nullptr : (uint4 *)c->nodesq4.p, (float *)c->qgrid.p);
     MCS_LAUNCH_CHECK();
     if (sah) {
-        if (int e = mcs_buf_reserve(c->sleft, nT * sizeof(int32_t), s)) return e;
-        if (int e = mcs_buf_reserve(c->sright, nT * sizeof(int32_t), s)) return e;
-        if (int e = mcs_buf_reserve(c->scnt, nT * sizeof(int32_t), s)) return e;
-        if (int e = mcs_buf_reserve(c->sbox, nT * 2 * sizeof(float4), s)) return e;
-        if (int e = mcs_buf_reserve(c->sfirst, nN * sizeof(int32_t), s)) return e;
-        if (int e = mcs_buf_reserve(c->swork, nT * (4 * sizeof(float4) + 4 * sizeof(int32_t)), s)) return e;
-        if (int e = mcs_buf_reserve(c->stris, nT * 3 * sizeof(float4), s)) return e;
         const ShadowTree st{(int32_t *)c->sleft.p, (int32_t *)c->sright.p, (float4 *)c->sbox.p, (int32_t *)c->scnt.p, (int32_t *)c->sfirst.p};
-        float4 *cbox = (float4 *)c->swork.p;                      // [2][T][2]
-        int32_t *cid = (int32_t *)(cbox + 4 * nT);                // [2][T]
-        k_ploc<<<1, PLOC_THREADS, 0, s>>>(T, (const float *)c->lo.p, (const float *)c->hi.p, st, cid, cbox, cid + 2 * nT, cid + 3 * nT);
+        k_ploc<<<1, PLOC_THREADS, 0, s>>>(T, (const float *)c->lo.p, (const float *)c->hi.p, st, (int32_t *)c->cid.p, (float4 *)c->cbox.p,
+                                          (int32_t *)c->nn.p, (int32_t *)c->round_id.p);
         MCS_LAUNCH_CHECK();
         k_emit_shadow<<<nblk(T, 256), 256, 0, s>>>(T, st, (const float *)c->lo.p, (const float *)c->hi.p, (const float4 *)c->tris.p, (float4 *)c->stris.p,
                                                    (uint4 *)c->nodesq4.p);
         MCS_LAUNCH_CHECK();
     }
-    c->shadow_sah = sah;
     c->T = T; c->V = V;
     return 0;
 }
@@ -837,9 +818,9 @@ int mcs_bvh_export_shadow(mcs_ctx *c, uint32_t *nodesq4, float *tris, float *qgr
     cudaStream_t s = (cudaStream_t)stream;
     MCS_REQUIRE(c && c->T > 0, "mcs_bvh_export_shadow: no acceleration structure built");
     const size_t T = (size_t)c->T;
-    MCS_CUDA(cudaMemcpyAsync(nodesq4, c->nodesq4.p, (T > 1 ? T - 1 : 1) * 4 * sizeof(uint4), cudaMemcpyDeviceToDevice, s));
-    MCS_CUDA(cudaMemcpyAsync(tris, c->shadow_sah ? c->stris.p : c->tris.p, T * 3 * sizeof(float4), cudaMemcpyDeviceToDevice, s));
-    MCS_CUDA(cudaMemcpyAsync(qgrid, c->qgrid.p, 9 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    MCS_CUDA(cudaMemcpyAsync(nodesq4, c->shadow.nodesq4, (T > 1 ? T - 1 : 1) * 4 * sizeof(uint4), cudaMemcpyDeviceToDevice, s));
+    MCS_CUDA(cudaMemcpyAsync(tris, c->shadow.tris, T * 3 * sizeof(float4), cudaMemcpyDeviceToDevice, s));
+    MCS_CUDA(cudaMemcpyAsync(qgrid, c->shadow.qgrid, 9 * sizeof(float), cudaMemcpyDeviceToDevice, s));
     return 0;
 }
 

@@ -1109,8 +1109,8 @@ static int fill_params(mcs_ctx *ctx, EnvParams &p,
     p.perms = (const int32_t *)perms->ptr; p.pm_s1 = perms->strides[1]; p.pm_s3 = perms->strides[3]; p.n_perms = (uint32_t)perms->sizes[1];
     p.m_rows = cdf_iters(p.Hl); p.m_cols = cdf_iters(p.Wl);
     p.bsdf = bsdf; p.seed = rnd_seed; p.seed_dev = seed_offset_dev; p.batch_offset = batch_offset; p.shadow_scale = shadow_scale;
-    p.bvh = BvhView{(const float4 *)ctx->nodes.p, (const float4 *)(ctx->shadow_sah ? ctx->stris.p : ctx->tris.p), (const float *)ctx->qgrid.p,
-                    (const uint4 *)ctx->nodesq4.p};
+    p.bvh = ctx->shadow;
+    p.bvh.nodes = (const float4 *)ctx->nodes.p;
     if (int e = ensure_skip_table(ctx, p.N, s, &p.skip)) return e;
     // work-claim counter of the persistent grid: one slot of a small ring PER LAUNCH, so launches of the same context that are in
     // flight on different streams never share a counter

@@ -67,6 +67,11 @@ int mcs_trace_visibility(mcs_ctx *ctx, const float *ro, const float *rd, int64_t
  * tri_id[i] = original triangle id or -1; tuv[i] = (t, u, v). */
 int mcs_trace_closest(mcs_ctx *ctx, const float *ro, const float *rd, int64_t n, int32_t *tri_id, float *tuv, mcs_stream stream);
 
+/* Closest hit beyond a per-ray bound (the ray-level form of depth peeling, see mcs_rasterize_peel): only hits with
+ * t > sep(t_after[i]) count, sep(t) = fl32(t * (1 + 2^-16)); t_after[i] = +inf gives a miss.  Outputs as mcs_trace_closest. */
+int mcs_trace_closest_after(mcs_ctx *ctx, const float *ro, const float *rd, const float *t_after, int64_t n, int32_t *tri_id, float *tuv,
+                            mcs_stream stream);
+
 /* ---- fused env-light importance sampling + shadow rays + BSDF:
  *      replaces env_shade_fwd / env_shade_bwd, optixutils/c_src/torch_bindings.cpp:123-188 / 190-272
  *      (optixLaunch of __raygen__rg, envsampling/kernel.cu:463-542).
@@ -213,6 +218,13 @@ int mcs_shade_combine_bwd(const mcs_tensor *a4, const mcs_tensor *b4, const mcs_
  *      interpolate: attr [V,C] (attr_batch_stride 0) or [B,V,C] (stride V*C), tris int32 [T,3], out / d_out [B,H,W,C];
  *      d_attr (same layout as attr) must be zeroed by the caller and receives float atomics. */
 int mcs_rasterize(mcs_ctx *ctx, const float *mtx, int32_t B, int32_t H, int32_t W, float *rast, mcs_stream stream);
+/* Depth peeling, the stand-in for dr.DepthPeeler (render/render.py:308-311): one layer per call.  t_state: [B,H,W] fp32 device array,
+ * in/out, zero-filled by the caller before layer 0; it holds each pixel's last hit t along the un-projected near-far segment, or +inf
+ * once the pixel is exhausted.  Layer k+1 is the closest hit with t > sep(t_prev), sep(t) = fl32(t * (1 + 2^-16)): surfaces closer
+ * than that along the ray merge into one layer, so a ray through a shared edge does not return the same surface twice.  Layer 0 equals
+ * mcs_rasterize bit for bit; an exhausted pixel is all zeros.  rast as mcs_rasterize.  No host sync (a peel loop can be captured in a
+ * CUDA graph); the BVH must not be rebuilt or refitted between the layers of one peel. */
+int mcs_rasterize_peel(mcs_ctx *ctx, const float *mtx, int32_t B, int32_t H, int32_t W, float *t_state, float *rast, mcs_stream stream);
 int mcs_interpolate_fwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
                         int32_t B, int32_t H, int32_t W, float *out, mcs_stream stream);
 int mcs_interpolate_bwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,

@@ -78,6 +78,7 @@ _SIGS = {
     "mcs_bvh_export_shadow": ([_P] * 5, C.c_int),
     "mcs_trace_visibility": ([_P, _P, _P, C.c_int64, _P, _P], C.c_int),
     "mcs_trace_closest": ([_P, _P, _P, C.c_int64, _P, _P, _P], C.c_int),
+    "mcs_trace_closest_after": ([_P, _P, _P, _P, C.c_int64, _P, _P, _P], C.c_int),
     "mcs_env_shade_fwd": ([_P] + [_T] * 12 + [C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_float, C.c_int32, _P, _P, _P, _P, _P, C.c_int32, _P], C.c_int),
     "mcs_env_shade_bwd_replay": ([_T] * 6 + [C.c_uint32, C.c_uint32, C.c_float, _T, _T, _P, _P, C.c_int32] + [_P] * 6, C.c_int),
     "mcs_env_shade_records": ([_P] + [_T] * 12 + [C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_float, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
@@ -115,6 +116,7 @@ _SIGS = {
     "mcs_texel_fetch_fwd": ([_P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P], C.c_int),
     "mcs_texel_fetch_bwd": ([C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, _P], C.c_int),
     "mcs_rasterize": ([_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
+    "mcs_rasterize_peel": ([_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
     "mcs_interpolate_fwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
     "mcs_interpolate_bwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
     "mcs_interpolate_bwd_rast": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P], C.c_int),
@@ -151,7 +153,8 @@ def lib():
 # kernels: bounds init, triangle bounds, Morton codes, radix sort (histogram + 4 passes), Karras topology, leaves + refit, node emission,
 # and for meshes of 5 to 16 384 triangles the shadow view's clustering and emission.
 LAUNCHES = collections.Counter()
-_KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "antialias_topology": 2}
+_KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "rasterize_peel": 2,
+                     "antialias_topology": 2}
 
 
 def check(status, what):

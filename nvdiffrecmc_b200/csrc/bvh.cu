@@ -697,14 +697,17 @@ __global__ void __launch_bounds__(128) k_visibility(VisView b, const float *__re
     vis[i] = bvh_occluded(b, o, d) ? 0 : 1;        // fp32 nodes, same triangles and predicate as the fused env_shade kernel
 }
 
-__global__ void __launch_bounds__(128) k_closest(BvhView b, const float *__restrict__ ro, const float *__restrict__ rd, int64_t n,
-                                                 int32_t *__restrict__ tri_id, float *__restrict__ tuv)
+// AFTER: only hits with t > peel_sep(t_after[i]) count.  +inf gives a miss: every box's clamped entry is +inf, so the walk ends after
+// the root.  A template parameter rather than a null test, so that the plain query keeps its constant bound (46 registers, not 47).
+template <bool AFTER>
+__global__ void __launch_bounds__(128) k_closest(BvhView b, const float *__restrict__ ro, const float *__restrict__ rd, const float *__restrict__ t_after,
+                                                 int64_t n, int32_t *__restrict__ tri_id, float *__restrict__ tuv)
 {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     f3 o = F3(ro[3 * i], ro[3 * i + 1], ro[3 * i + 2]), d = F3(rd[3 * i], rd[3 * i + 1], rd[3 * i + 2]);
     float t, u, v;
-    int id = bvh_closest(b, o, d, t, u, v);
+    int id = bvh_closest(b, o, d, AFTER ? peel_sep(t_after[i]) : 0.0f, t, u, v);
     tri_id[i] = id; tuv[3 * i] = t; tuv[3 * i + 1] = u; tuv[3 * i + 2] = v;
 }
 
@@ -841,7 +844,19 @@ int mcs_trace_closest(mcs_ctx *c, const float *ro, const float *rd, int64_t n, i
     MCS_REQUIRE(n >= 0 && (n == 0 || (ro && rd && tri_id && tuv)), "mcs_trace_closest: bad arguments");
     if (n == 0) return 0;
     BvhView b{(const float4 *)c->nodes.p, (const float4 *)c->tris.p, nullptr, nullptr};
-    k_closest<<<nblk(n, 128), 128, 0, (cudaStream_t)stream>>>(b, ro, rd, n, tri_id, tuv);
+    k_closest<false><<<nblk(n, 128), 128, 0, (cudaStream_t)stream>>>(b, ro, rd, nullptr, n, tri_id, tuv);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_trace_closest_after(mcs_ctx *c, const float *ro, const float *rd, const float *t_after, int64_t n, int32_t *tri_id, float *tuv,
+                            mcs_stream stream)
+{
+    MCS_REQUIRE(c && c->T > 0, "mcs_trace_closest_after: no acceleration structure built (call mcs_bvh_build first)");
+    MCS_REQUIRE(n >= 0 && (n == 0 || (ro && rd && t_after && tri_id && tuv)), "mcs_trace_closest_after: bad arguments");
+    if (n == 0) return 0;
+    BvhView b{(const float4 *)c->nodes.p, (const float4 *)c->tris.p, nullptr, nullptr};
+    k_closest<true><<<nblk(n, 128), 128, 0, (cudaStream_t)stream>>>(b, ro, rd, t_after, n, tri_id, tuv);
     MCS_LAUNCH_CHECK();
     return 0;
 }

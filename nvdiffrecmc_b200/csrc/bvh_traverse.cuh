@@ -23,8 +23,8 @@ struct BvhView {
 };
 
 // Moeller-Trumbore with a fixed evaluation order (mirrors oracle mt_hit()).  Returns true on a hit
-// with t in (0, tmax); u, v, t are written on a hit.
-__device__ __forceinline__ bool mt_hit(f3 o, f3 d, f3 v0, f3 e1, f3 e2, float tmax, float &t_out, float &u_out, float &v_out)
+// with t in (tmin, tmax), tmin >= 0; u, v, t are written on a hit.
+__device__ __forceinline__ bool mt_hit(f3 o, f3 d, f3 v0, f3 e1, f3 e2, float tmax, float &t_out, float &u_out, float &v_out, float tmin = 0.0f)
 {
     float px = __fmaf_rn(d.y, e2.z, -__fmul_rn(d.z, e2.y));
     float py = __fmaf_rn(d.z, e2.x, -__fmul_rn(d.x, e2.z));
@@ -41,7 +41,7 @@ __device__ __forceinline__ bool mt_hit(f3 o, f3 d, f3 v0, f3 e1, f3 e2, float tm
     float v = __fmul_rn(__fmaf_rn(d.x, qx, __fmaf_rn(d.y, qy, __fmul_rn(d.z, qz))), inv);
     if (v < 0.0f || __fadd_rn(u, v) > 1.0f) return false;
     float t = __fmul_rn(__fmaf_rn(e2.x, qx, __fmaf_rn(e2.y, qy, __fmul_rn(e2.z, qz))), inv);
-    if (!(t > 0.0f && t < tmax)) return false;
+    if (!(t > tmin && t < tmax)) return false;
     t_out = t; u_out = u; v_out = v;
     return true;
 }
@@ -60,6 +60,12 @@ __device__ __forceinline__ RayPre ray_pre(f3 o, f3 d)
     r.ox = o.x * r.ix; r.oy = o.y * r.iy; r.oz = o.z * r.iz;
     return r;
 }
+
+// Depth-peeling separation: the next layer along a ray is the closest hit with t > peel_sep(t_prev), one exactly rounded fp32
+// multiply by 1 + 2^-16 (exact in fp32, about 128 ulp of t).  A plain t > t_prev would return the same surface again where a ray
+// crosses a shared edge: Moeller-Trumbore's closed bounds accept it on both triangles at t values a few ulp apart.  Surfaces closer
+// than this along the ray merge into one layer, as nvdiffrast's peeler drops fragments at equal depth.  tests/peel_oracle.c restates it.
+__device__ __forceinline__ float peel_sep(float t) { return __fmul_rn(t, 1.0000152587890625f); }
 
 #define MCS_STACK 64
 #define MCS_LEAF_MAX 4
@@ -112,8 +118,12 @@ __device__ __forceinline__ bool bvh_occluded(const BvhView &b, f3 o, f3 d)
 }
 
 // Closest-hit query (primary rays of the synthetic G-buffer producer).  Ties in t are resolved
-// towards the smaller original triangle id, matching the oracle's brute-force scan.
-__device__ __forceinline__ int bvh_closest(const BvhView &b, f3 o, f3 d, float &t_best, float &u_best, float &v_best)
+// towards the smaller original triangle id, matching the oracle's brute-force scan.  Only hits with
+// t > t_lo count (t_lo = 0: every hit mt_hit accepts; depth peeling passes the previous layer's
+// separated t).  t_lo enters as the lower clamp of each box's entry distance, so a box is skipped
+// for it only when its relaxed exit distance lies strictly before t_lo: the culling stays as
+// conservative as the t_best bound, and with t_lo = 0 the code is the plain closest-hit walk.
+__device__ __forceinline__ int bvh_closest(const BvhView &b, f3 o, f3 d, float t_lo, float &t_best, float &u_best, float &v_best)
 {
     const RayPre r = ray_pre(o, d);
     int stack[MCS_STACK];
@@ -128,12 +138,12 @@ __device__ __forceinline__ int bvh_closest(const BvhView &b, f3 o, f3 d, float &
             float a0 = fmaf(q0.x, r.ix, -r.ox), a1 = fmaf(q0.y, r.ix, -r.ox);
             float b0 = fmaf(q0.z, r.iy, -r.oy), b1 = fmaf(q0.w, r.iy, -r.oy);
             float c0 = fmaf(q2.x, r.iz, -r.oz), c1 = fmaf(q2.y, r.iz, -r.oz);
-            float tn0 = fmaxf(fmaxf(fminf(a0, a1), fminf(b0, b1)), fmaxf(fminf(c0, c1), 0.0f));
+            float tn0 = fmaxf(fmaxf(fminf(a0, a1), fminf(b0, b1)), fmaxf(fminf(c0, c1), t_lo));
             float tf0 = fminf(fminf(fmaxf(a0, a1), fmaxf(b0, b1)), fminf(fmaxf(c0, c1), t_best));
             a0 = fmaf(q1.x, r.ix, -r.ox); a1 = fmaf(q1.y, r.ix, -r.ox);
             b0 = fmaf(q1.z, r.iy, -r.oy); b1 = fmaf(q1.w, r.iy, -r.oy);
             c0 = fmaf(q2.z, r.iz, -r.oz); c1 = fmaf(q2.w, r.iz, -r.oz);
-            float tn1 = fmaxf(fmaxf(fminf(a0, a1), fminf(b0, b1)), fmaxf(fminf(c0, c1), 0.0f));
+            float tn1 = fmaxf(fmaxf(fminf(a0, a1), fminf(b0, b1)), fmaxf(fminf(c0, c1), t_lo));
             float tf1 = fminf(fminf(fmaxf(a0, a1), fmaxf(b0, b1)), fminf(fmaxf(c0, c1), t_best));
             const bool h0 = tn0 <= tf0 * 1.0000004f + 1e-30f, h1 = tn1 <= tf1 * 1.0000004f + 1e-30f;
             const int ch0 = __float_as_int(q3.x), ch1 = __float_as_int(q3.y);
@@ -153,7 +163,7 @@ __device__ __forceinline__ int bvh_closest(const BvhView &b, f3 o, f3 d, float &
                 const float4 t0 = __ldg(t), t1 = __ldg(t + 1), t2 = __ldg(t + 2);
                 float tt, uu, vv;
                 // exact ties in t are resolved by the original triangle id (brute-force order)
-                if (mt_hit(o, d, F3(t0.x, t0.y, t0.z), F3(t1.x, t1.y, t1.z), F3(t2.x, t2.y, t2.z), MCS_TMAX, tt, uu, vv)) {
+                if (mt_hit(o, d, F3(t0.x, t0.y, t0.z), F3(t1.x, t1.y, t1.z), F3(t2.x, t2.y, t2.z), MCS_TMAX, tt, uu, vv, t_lo)) {
                     const int id = __float_as_int(t0.w);
                     if (tt < t_best || (tt == t_best && id < best)) { t_best = tt; u_best = uu; v_best = vv; best = id; }
                 }

@@ -6,6 +6,16 @@
 //                   Moeller-Trumbore predicate as the shadow rays, ties broken by triangle id), and the result is written in
 //                   nvdiffrast's `rast` convention: (u, v, z/w, triangle_id + 1), u / v = barycentric weights of vertex 0 / 1,
 //                   0 in all channels for background.  Image row iy maps to NDC y = (iy + 0.5) / H * 2 - 1 (no flip, like dr.rasterize).
+//                   Depth peeling (render/render.py:308-311 takes every layer from dr.DepthPeeler) is the same launch given a per-pixel
+//                   state t_state [B,H,W], zero before layer 0, where t is measured along d = far - near:
+//                     - layer k+1 is the closest hit with t > sep(t_prev), sep(t) = fl32(t * (1 + 2^-16)) (peel_sep, bvh_traverse.cuh),
+//                       ties in t to the smaller triangle id, written as (u, v, z/w, id + 1) like any rast;
+//                     - the state becomes that hit's t, or +inf when there is none; a +inf pixel writes zeros and skips traversal;
+//                     - t_prev = 0 gives sep = 0 and mt_hit already requires t > 0, so layer 0 equals rasterize bit for bit.
+//                   The separation is a deliberate choice: Moeller-Trumbore's closed bounds make a ray through a shared edge hit both
+//                   triangles a few ulp apart, and a plain t > t_prev would return that surface again as a spurious layer.  Surfaces
+//                   closer than 2^-16 t (about 128 ulp) along the ray merge into one layer.  Each layer is an ordinary rast: the
+//                   backward below and antialias take it unchanged.
 //   k_interpolate : out[b,y,x,:] = u * A[i0] + v * A[i1] + (1 - u - v) * A[i2]; backward scatters into dA with float atomics and, when
 //                   the caller asks for it, writes d rast[...,0:2] = (sum_c g_c (A0_c - A2_c), sum_c g_c (A1_c - A2_c)) (one writer per pixel).
 //
@@ -53,6 +63,7 @@ struct RasterParams {
     const float *mtx, *inv;      // [B,4,4] row-major, clip = mtx * (p, 1)
     int B, H, W;
     float *rast;
+    float *t_state;              // [B,H,W] depth-peeling state (t of the last layer's hit, +inf when exhausted), or null for plain rasterize
 };
 
 __device__ __forceinline__ void mul4(const float *__restrict__ m, float x, float y, float z, float w, float (&o)[4])
@@ -74,8 +85,14 @@ __global__ void __launch_bounds__(128) k_rasterize(const RasterParams p)
     const f3 o = F3(a[0] / a[3], a[1] / a[3], a[2] / a[3]);
     const f3 f = F3(c[0] / c[3], c[1] / c[3], c[2] / c[3]);
     const f3 d = f - o;
+    float t_lo = 0.0f;
+    if (p.t_state) {
+        const float t_prev = p.t_state[i];
+        if (t_prev == INFINITY) { reinterpret_cast<float4 *>(p.rast)[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f); return; }
+        t_lo = peel_sep(t_prev);
+    }
     float t, u, v;
-    const int id = bvh_closest(p.bvh, o, d, t, u, v);
+    const int id = bvh_closest(p.bvh, o, d, t_lo, t, u, v);
     float4 out = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     if (id >= 0) {
         const f3 h = o + d * t;
@@ -84,6 +101,7 @@ __global__ void __launch_bounds__(128) k_rasterize(const RasterParams p)
         out = make_float4(1.0f - u - v, u, q[2] / q[3], (float)(id + 1));
     }
     reinterpret_cast<float4 *>(p.rast)[i] = out;
+    if (p.t_state) p.t_state[i] = id >= 0 ? t : INFINITY;
 }
 
 // inverse of B row-major 4x4 matrices, Gauss-Jordan with partial pivoting in fp64 (one thread per matrix; a singular matrix gives NaNs,
@@ -494,21 +512,33 @@ __global__ void __launch_bounds__(256) k_texel_fetch(const float *__restrict__ t
 
 extern "C" {
 
-int mcs_rasterize(mcs_ctx *c, const float *mtx, int32_t B, int32_t H, int32_t W, float *rast, mcs_stream stream)
+static int rasterize_launch(mcs_ctx *c, const float *mtx, int32_t B, int32_t H, int32_t W, float *t_state, float *rast, mcs_stream stream)
 {
-    MCS_REQUIRE(c && c->T > 0, "mcs_rasterize: no acceleration structure built (call mcs_bvh_build first)");
-    MCS_REQUIRE(mtx && rast && B > 0 && H > 0 && W > 0, "mcs_rasterize: bad arguments");
     if (int e = mcs_buf_reserve(c->mtx_inv, sizeof(float) * 16 * (size_t)B, (cudaStream_t)stream)) return e;
     float *inv_mtx = (float *)c->mtx_inv.p;
     k_invert4<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(mtx, inv_mtx, B);
     MCS_LAUNCH_CHECK();
     RasterParams p{};
     p.bvh = BvhView{(const float4 *)c->nodes.p, (const float4 *)c->tris.p, nullptr, nullptr};
-    p.mtx = mtx; p.inv = inv_mtx; p.B = B; p.H = H; p.W = W; p.rast = rast;
+    p.mtx = mtx; p.inv = inv_mtx; p.B = B; p.H = H; p.W = W; p.rast = rast; p.t_state = t_state;
     const int64_t n = (int64_t)B * H * W;
     k_rasterize<<<(unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream>>>(p);
     MCS_LAUNCH_CHECK();
     return 0;
+}
+
+int mcs_rasterize(mcs_ctx *c, const float *mtx, int32_t B, int32_t H, int32_t W, float *rast, mcs_stream stream)
+{
+    MCS_REQUIRE(c && c->T > 0, "mcs_rasterize: no acceleration structure built (call mcs_bvh_build first)");
+    MCS_REQUIRE(mtx && rast && B > 0 && H > 0 && W > 0, "mcs_rasterize: bad arguments");
+    return rasterize_launch(c, mtx, B, H, W, nullptr, rast, stream);
+}
+
+int mcs_rasterize_peel(mcs_ctx *c, const float *mtx, int32_t B, int32_t H, int32_t W, float *t_state, float *rast, mcs_stream stream)
+{
+    MCS_REQUIRE(c && c->T > 0, "mcs_rasterize_peel: no acceleration structure built (call mcs_bvh_build first)");
+    MCS_REQUIRE(mtx && t_state && rast && B > 0 && H > 0 && W > 0, "mcs_rasterize_peel: bad arguments");
+    return rasterize_launch(c, mtx, B, H, W, t_state, rast, stream);
 }
 
 static int interp_common(InterpParams &p, const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T,

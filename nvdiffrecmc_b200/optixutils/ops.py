@@ -245,14 +245,23 @@ def trace_visibility(optix_ctx, ro, rd):
     return vis
 
 
-def trace_closest(optix_ctx, ro, rd):
-    """(tri_id int32 [n] (-1 = miss), tuv fp32 [n,3] = (t, u, v))"""
+def trace_closest(optix_ctx, ro, rd, t_after=None):
+    """(tri_id int32 [n] (-1 = miss), tuv fp32 [n,3] = (t, u, v)).  t_after (fp32 [n], optional): only hits with
+    t > t_after * (1 + 2^-16) count, +inf gives a miss -- one ray of a depth peel (raster.DepthPeeler), t_after the previous hit's t."""
     L.require_cuda(ro, rd)
     ro = _f32(ro, "ro").reshape(-1, 3).contiguous(); rd = _f32(rd, "rd").reshape(-1, 3).contiguous()
     tid = torch.empty(ro.shape[0], dtype=torch.int32, device=ro.device)
     tuv = torch.empty(ro.shape[0], 3, dtype=torch.float32, device=ro.device)
-    L.check(L.lib().mcs_trace_closest(optix_ctx.cpp_wrapper, ro.data_ptr(), rd.data_ptr(), ro.shape[0], tid.data_ptr(), tuv.data_ptr(),
-                                      L.stream_ptr()), "trace_closest")
+    if t_after is None:
+        L.check(L.lib().mcs_trace_closest(optix_ctx.cpp_wrapper, ro.data_ptr(), rd.data_ptr(), ro.shape[0], tid.data_ptr(), tuv.data_ptr(),
+                                          L.stream_ptr()), "trace_closest")
+        return tid, tuv
+    L.require_cuda(t_after)
+    ta = _f32(t_after, "t_after").reshape(-1).contiguous()
+    if ta.shape[0] != ro.shape[0]:
+        raise ValueError("trace_closest: t_after has %d entries for %d rays" % (ta.shape[0], ro.shape[0]))
+    L.check(L.lib().mcs_trace_closest_after(optix_ctx.cpp_wrapper, ro.data_ptr(), rd.data_ptr(), ta.data_ptr(), ro.shape[0], tid.data_ptr(),
+                                            tuv.data_ptr(), L.stream_ptr()), "trace_closest")
     return tid, tuv
 
 

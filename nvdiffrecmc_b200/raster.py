@@ -6,8 +6,9 @@ already built for the shadow rays and returns nvdiffrast's `rast` tensor `(u, v,
 vertices `pos` it is differentiable with respect to them through the barycentrics.  `interpolate` evaluates vertex attributes at
 those barycentrics and is differentiable with respect to the attributes and to `rast`.  `antialias` is the pixel-pair analytic
 antialiasing of Laine et al. 2020, the only path from coverage (alpha) to vertex positions, so silhouette losses train the mesh;
-`antialias_topology` builds the edge adjacency it needs on the device.  Screen-space derivatives (`rast_db`, `diff_attrs`) are not
-provided."""
+`antialias_topology` builds the edge adjacency it needs on the device.  `DepthPeeler` returns the deeper layers of the same G-buffer
+(the next surface along each primary ray), each an ordinary `rast` that `interpolate` and `antialias` take, as render_mesh's
+back-to-front `composite_buffer` needs.  Screen-space derivatives (`rast_db`, `diff_attrs`) are not provided."""
 import torch
 from . import _lib as L
 
@@ -30,17 +31,21 @@ def _check_tri(tri, name, what="tri"):
         raise ValueError("%s: %s must be a non-empty [T,3], got %s" % (name, what, tuple(tri.shape)))
 
 
-def _rasterize_launch(optix_ctx, m, resolution):
+def _rasterize_launch(optix_ctx, m, resolution, t_state=None):
     B, (H, W) = m.shape[0], resolution
     rast = torch.empty(B, H, W, 4, dtype=torch.float32, device=m.device)
-    L.check(L.lib().mcs_rasterize(optix_ctx.cpp_wrapper, m.data_ptr(), B, H, W, rast.data_ptr(), L.stream_ptr()), "rasterize")
+    if t_state is None:
+        L.check(L.lib().mcs_rasterize(optix_ctx.cpp_wrapper, m.data_ptr(), B, H, W, rast.data_ptr(), L.stream_ptr()), "rasterize")
+    else:
+        L.check(L.lib().mcs_rasterize_peel(optix_ctx.cpp_wrapper, m.data_ptr(), B, H, W, t_state.data_ptr(), rast.data_ptr(), L.stream_ptr()),
+                "rasterize_peel")
     return rast
 
 
 class _rasterize_func(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, pos, tri, optix_ctx, m, resolution):
-        rast = _rasterize_launch(optix_ctx, m, resolution)
+    def forward(ctx, pos, tri, optix_ctx, m, resolution, t_state=None):
+        rast = _rasterize_launch(optix_ctx, m, resolution, t_state)
         ctx.save_for_backward(pos, tri, rast)
         return rast
 
@@ -53,7 +58,25 @@ class _rasterize_func(torch.autograd.Function):
         V = pos.shape[-2]
         L.check(L.lib().mcs_rasterize_bwd(pos.data_ptr(), V * 4 if pos.dim() == 3 else 0, V, tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W,
                                           g.data_ptr(), d_pos.data_ptr(), L.stream_ptr()), "rasterize (backward)")
-        return d_pos, None, None, None, None
+        return d_pos, None, None, None, None, None
+
+
+def _rasterize_args(name, mtx, pos, tri):
+    """Validated (contiguous fp32 mtx, pos, tri) of a rasterize-style call; pos and tri are None together."""
+    L.require_cuda(mtx)
+    if mtx.dim() != 3 or mtx.shape[1:] != (4, 4):
+        raise ValueError("%s: mtx must be [B,4,4]" % name)
+    m = mtx.detach().to(torch.float32).contiguous()
+    if pos is None:
+        if tri is not None:
+            raise ValueError("%s: tri is only used together with pos" % name)
+        return m, None, None
+    if tri is None:
+        raise ValueError("%s: pos needs tri" % name)
+    L.require_cuda(pos, tri)
+    _check_pos(pos, m.shape[0], name)
+    _check_tri(tri, name)
+    return m, pos.contiguous(), tri.contiguous()
 
 
 def rasterize(optix_ctx, mtx, resolution, pos=None, tri=None):
@@ -64,20 +87,52 @@ def rasterize(optix_ctx, mtx, resolution, pos=None, tri=None):
     `ru.xfm_points(v_pos[None], mtx)`) and tri (int32 [T,3]) make the result differentiable with respect to pos: the forward is the
     same ray-traced launch with a bit-identical output, and the backward maps d rast[...,0:2] to d pos through the perspective-correct
     barycentrics of the clip-space triangle.  z/w and the id channel carry no gradient."""
-    L.require_cuda(mtx)
-    if mtx.dim() != 3 or mtx.shape[1:] != (4, 4):
-        raise ValueError("rasterize: mtx must be [B,4,4]")
-    m = mtx.detach().to(torch.float32).contiguous()
+    m, pos, tri = _rasterize_args("rasterize", mtx, pos, tri)
     if pos is None:
-        if tri is not None:
-            raise ValueError("rasterize: tri is only used together with pos")
         return _rasterize_launch(optix_ctx, m, resolution)
-    if tri is None:
-        raise ValueError("rasterize: pos needs tri")
-    L.require_cuda(pos, tri)
-    _check_pos(pos, m.shape[0], "rasterize")
-    _check_tri(tri, "rasterize")
-    return _rasterize_func.apply(pos.contiguous(), tri.contiguous(), optix_ctx, m, resolution)
+    return _rasterize_func.apply(pos, tri, optix_ctx, m, resolution)
+
+
+class DepthPeeler:
+    """Depth peeling, the stand-in for nvdiffrast's `dr.DepthPeeler` in render_mesh (render/render.py:308-311).  Arguments as
+    `rasterize`; use it as a context manager:
+
+        with DepthPeeler(optix_ctx, mtx, (H, W), pos, tri) as peeler:
+            for _ in range(num_layers):
+                rast, _ = peeler.rasterize_next_layer()
+
+    Each layer is the next surface along every pixel's primary ray: the closest hit with t > t_prev * (1 + 2^-16) in fp32, where
+    t_prev is the previous layer's hit (semantics in csrc/raster.cu).  Surfaces closer than that along the ray merge into one layer,
+    so a ray through an edge shared by two triangles does not return the same surface twice.  Layer 0 equals `rasterize`; a pixel
+    with no further surface is all zeros.  Every layer is an ordinary `rast`: given pos and tri it is differentiable with respect to
+    pos exactly like `rasterize`, and `interpolate` and `antialias` take it.  The peeler keeps one fp32 per pixel, zeroed on entry.
+    Rebuilding or refitting the context's BVH between layers is an error, as it is for nvdiffrast's peeler to change the geometry."""
+
+    def __init__(self, optix_ctx, mtx, resolution, pos=None, tri=None):
+        self._m, self._pos, self._tri = _rasterize_args("DepthPeeler", mtx, pos, tri)
+        self._ctx, self._res = optix_ctx, tuple(resolution)
+        self._state = None
+        self._version = None
+
+    def __enter__(self):
+        H, W = self._res
+        self._state = torch.zeros(self._m.shape[0], H, W, dtype=torch.float32, device=self._m.device)
+        self._version = self._ctx._version
+        return self
+
+    def __exit__(self, *exc):
+        self._state = None
+        return False
+
+    def rasterize_next_layer(self):
+        """Returns (rast [B,H,W,4], None), like dr.DepthPeeler.rasterize_next_layer without screen-space derivatives."""
+        if self._state is None:
+            raise RuntimeError("DepthPeeler.rasterize_next_layer: only inside the peeler's `with` block")
+        if self._ctx._version != self._version:
+            raise RuntimeError("DepthPeeler.rasterize_next_layer: the BVH was rebuilt or refitted since the peeler started")
+        if self._pos is None:
+            return _rasterize_launch(self._ctx, self._m, self._res, self._state), None
+        return _rasterize_func.apply(self._pos, self._tri, self._ctx, self._m, self._res, self._state), None
 
 
 class _interpolate_func(torch.autograd.Function):
@@ -165,7 +220,7 @@ class _antialias_func(torch.autograd.Function):
 
 def antialias(color, rast, pos, tri, topology=None):
     """Analytic antialiasing of `color` [B,H,W,C] (any C >= 1) along silhouette edges, the stand-in for dr.antialias in render_mesh's
-    composite_buffer (render/render.py:290).  rast from `rasterize`, pos the clip-space vertices [V,4] or [B,V,4] it was made from,
+    composite_buffer (render/render.py:290).  rast from `rasterize` or a `DepthPeeler` layer, pos the clip-space vertices [V,4] or [B,V,4] it was made from,
     tri int32 [T,3], topology from `antialias_topology(tri)` (built inside the call when None; pass it to share one build between
     the buffers of a frame).  Differentiable with respect to color and pos; rast carries no gradient.  The output is a
     deterministic per-pixel gather and antialias is linear in color for fixed geometry, so channels of several buffers may be

@@ -55,6 +55,13 @@ rg = rasterize(ctx, mg, (24, 24), pos=posg, tri=t("tris"))
 ig, _ = interpolate(t("verts"), rg, t("tris"))
 antialias(torch.cat([ig, rg[..., 3:4].clamp(0, 1)], -1), rg, posg, t("tris")).sum().backward()
 antialias(torch.rand(1, 24, 24, 1, device=dev), rg.detach(), posg.detach()[0], t("tris"), antialias_topology(t("tris")))
+# depth peeling: three layers with a backward through each, and the ray-level query beyond a bound
+from nvdiffrecmc_b200.raster import DepthPeeler
+posp = posg.detach().clone().requires_grad_(True)
+with DepthPeeler(ctx, mg, (24, 24), posp, t("tris")) as peeler:
+    layers = [peeler.rasterize_next_layer()[0] for _ in range(3)]
+sum(antialias(rl[..., 3:4].clamp(0, 1), rl, posp, t("tris")).sum() + rl[..., :2].sum() for rl in layers).backward()
+ou.trace_closest(ctx, t("ro").reshape(-1, 3), torch.randn(c["ro"].size // 3, 3, device=dev), t_after=torch.rand(c["ro"].size // 3, device=dev))
 if os.environ.get("MCS_EW_TMA"):
     B, H, W = 1, 400, 400          # 160 000 px = 312 tiles of 512 px (>= 2 x 132) + a ragged tail
     ins = [torch.rand(B, H, W, 3, device=dev).requires_grad_(True) for _ in range(6)]

@@ -44,6 +44,10 @@ __device__ __forceinline__ float rsqrt_approx(float x) { float y; asm("rsqrt.app
 // 1 / max(dz * dist, 1e-4) = min(inv_dz * rsqrt(dist^2), 1e4) with inv_dz = dz > 0 ? 1/dz : +inf  (dist = 0 -> inf -> 1e4 as well)
 __device__ __forceinline__ float guarded_inv(float dz) { return dz > 0.0f ? 1.0f / dz : INFINITY; }
 
+// denoising.cu:26,86 filter_rad: the literal 2.5 is a double, so sigma * 2.5 is rounded in double, not fp32.  The two differ whenever the
+// fp32 product rounds down onto an integer: sigma = 3.2f is 3.2000000477, 8.0000001192 in double (r = 19) but exactly 8.0f in fp32 (r = 17).
+static int filter_radius(float sigma) { return 2 * (int)ceil((double)sigma * 2.5) + 1; }
+
 __device__ __forceinline__ float pow128(float x)
 {
     x *= x; x *= x; x *= x; x *= x; x *= x; x *= x; x *= x;
@@ -331,7 +335,7 @@ static int launch_bilateral_tma(const mcs_tensor *nrm, const mcs_tensor *zdz, co
     if (disabled || tma_encoder() == nullptr) return 1;
     if (!(tma_ok(nrm, 3) && tma_ok(zdz, 2) && tma_ok(sigA, CS) && (NSIG == 1 || tma_ok(sigB, CS)))) return 1;
     BilateralTmaParams p{};
-    p.r = 2 * (int)ceilf(sigma * 2.5f) + 1;
+    p.r = filter_radius(sigma);
     p.neg_inv_2var_log2e = -LOG2E / (2.0f * sigma * sigma);
     p.B = nrm->sizes[0]; p.H = nrm->sizes[1]; p.W = nrm->sizes[2];
     p.rl = (p.r + 3) & ~3;
@@ -370,7 +374,7 @@ template <int NSIG, bool BWD>
 static int launch_bilateral(BilateralParams &p, float sigma, cudaStream_t stream)
 {
     MCS_REQUIRE(sigma > 0.0f, "bilateral: sigma must be > 0");
-    p.r = 2 * (int)ceilf(sigma * 2.5f) + 1;                 // denoising.cu:28 filter_rad
+    p.r = filter_radius(sigma);
     p.neg_inv_2var_log2e = -LOG2E / (2.0f * sigma * sigma);
     int tw = TILE_W + 2 * p.r, th = TILE_H + 2 * p.r;
     size_t smem = sizeof(float) * ((size_t)(5 + 3 * NSIG) * tw * th);

@@ -62,3 +62,59 @@ def make_case(res=32, B=1, N=4, mesh="blob+torus", level=2, light="random", ligh
     return dict(verts=v, tris=f, scene=scene, mask=mask, ro=ro, pos=pos, nrm=nrm.astype(np.float32), view=view.astype(np.float32),
                 kd=st("kd"), ks=st("ks"), depth=st("depth"), smooth_nrm=sn, tangent=tg, geom_nrm=gn,
                 light=base, pdf=pdf, rows=rows, cols=cols, perms=perms, N=N, B=B, res=res)
+
+
+# The renderutils ops with their oracle entry points:
+# name, oracle forward, oracle backward, input channels, output channels, extras (f0, i0, i1), oracle kwargs
+RU_OPS = [
+    ("lambert", "lambert", "lambert_bwd", [3, 3], 1, (0.0, 0, 0), {}),
+    ("frostbite", "frostbite_diffuse", "frostbite_diffuse_bwd", [3, 3, 3, 1], 1, (0.0, 0, 0), {}),
+    ("fresnel", "fresnel_shlick", "fresnel_shlick_bwd", [3, 3, 1], 3, (0.0, 0, 0), {}),
+    ("ndf", "ndf_ggx", "ndf_ggx_bwd", [1, 1], 1, (0.0, 0, 0), {}),
+    ("lambda", "lambda_ggx", "lambda_ggx_bwd", [1, 1], 1, (0.0, 0, 0), {}),
+    ("masking", "masking_smith", "masking_smith_bwd", [1, 1, 1], 1, (0.0, 0, 0), {}),
+    ("specular", "pbr_specular", "pbr_specular_bwd", [3, 3, 3, 3, 1], 3, (0.08, 0, 0), {"min_roughness": 0.08}),
+    ("bsdf", "pbr_bsdf", "pbr_bsdf_bwd", [3] * 6, 3, (0.08, 0, 0), {"min_roughness": 0.08, "bsdf": "lambert"}),
+    ("bsdf", "pbr_bsdf", "pbr_bsdf_bwd", [3] * 6, 3, (0.08, 1, 0), {"min_roughness": 0.08, "bsdf": "frostbite"}),
+    ("psn", "prepare_shading_normal", "prepare_shading_normal_bwd", [3] * 6, 3, (0.0, 1, 1), {"two_sided_shading": True, "opengl": True}),
+    ("psn", "prepare_shading_normal", "prepare_shading_normal_bwd", [3] * 6, 3, (0.0, 0, 0), {"two_sided_shading": False, "opengl": False}),
+]
+
+
+def ru_edge_inputs(chans, out_c):
+    """Renderutils inputs the reference tests never draw: zero vectors (safe-normalise guard), back-facing / grazing configurations,
+    roughness at both ends of its clamp range, negative and > 1 values.  Returns ([1,6,8,c] inputs, [1,6,8,out_c] upstream gradient).
+    Pixels (0,0) .. (0,2) hold 0, 1 and -1 in every channel, (1,0) and (1,1) hold 1e-6 and 1e4."""
+    g = np.random.default_rng(11)
+    shape = (1, 6, 8)
+    ins = [g.normal(size=shape + (c,)).astype(np.float32) * (3.0 if c == 3 else 1.0) for c in chans]
+    for a in ins:
+        a[0, 0, 0] = 0.0                      # all-zero vectors / scalars
+        a[0, 0, 1] = 1.0
+        a[0, 0, 2] = -1.0
+        a[0, 1, 0] = 1e-6
+        a[0, 1, 1] = 1e4
+    dout = g.uniform(size=shape + (out_c,)).astype(np.float32)
+    return ins, dout
+
+
+def env_shade_edge_case():
+    """An env_shade problem with pixels the synthetic scenes never contain: zero shading normal, camera behind the surface (NdotV < 0),
+    roughness 0 and 1 (min-roughness clamp), pure metal, black albedo, and a probe with a black row and black texels.
+    Returns the make_case dict with those edits (pdf / rows / cols rebuilt for the edited probe); c["edge_px"][k] is the (b, y, x)
+    index of edited pixel k: 0 zero normal, 1 flipped normal, 2-4 ks edits, 5-6 kd edits."""
+    N = 4
+    c = make_case(res=16, B=1, N=N, seed=4)
+    m = c["mask"][0] > 0
+    ys, xs = np.nonzero(m)
+    assert len(ys) > 40
+    nrm, kd, ks = c["nrm"].copy(), c["kd"].copy(), c["ks"].copy()
+    px = [(0, ys[k], xs[k]) for k in range(7)]
+    nrm[px[0]] = 0.0
+    nrm[px[1]] = -nrm[px[1]]                                  # back-facing shading normal
+    ks[px[2]] = [0.0, 0.0, 0.0]; ks[px[3]] = [0.0, 1.0, 1.0]; ks[px[4]] = [0.0, 0.08, 0.5]
+    kd[px[5]] = 0.0; kd[px[6]] = 1.0
+    light = c["light"].copy(); light[3] = 0.0; light[10, ::2] = 0.0
+    pdf, rows, cols = oracle().update_pdf(light)
+    c.update(nrm=nrm, kd=kd, ks=ks, light=light, pdf=pdf, rows=rows, cols=cols, edge_px=px)
+    return c

@@ -164,7 +164,6 @@ colB = torch.rand(B, H, W, 3, generator=g).to(dev)
 with torch.no_grad():
     ms_f2 = timed(lambda: ou.bilateral_denoiser2(col.detach(), colB, nrm, zdz, 2.0))
 out["bilateral_denoiser"] = {"shape": [B, H, W], "sigma": 2.0, "taps_per_px": 529, "fwd_ms": round(ms_f, 4), "fwd2_ms_two_signals": round(ms_f2, 4), "bwd_ms": round(ms_b, 4),
-                             "fwd_path": "plain (MCS_DENOISE_NO_TMA)" if os.environ.get("MCS_DENOISE_NO_TMA") else "TMA-staged",
                              "fwd_gtaps_per_s": round(taps / ms_f / 1e6, 1), "fwd_gbs_compulsory_48B_per_px": round(B * H * W * 48 / ms_f / 1e6, 1)}
 print(out["bilateral_denoiser"], flush=True)
 

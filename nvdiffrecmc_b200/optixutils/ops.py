@@ -193,14 +193,14 @@ class _optix_env_shade_func(torch.autograd.Function):
                                                      C.byref(dg), C.byref(sg), rec_cnt.data_ptr(), rec_rays.data_ptr(), int(slots),
                                                      g[0].data_ptr(), g[1].data_ptr(), g[2].data_ptr(), g[3].data_ptr(), light_grad.data_ptr(),
                                                      L.stream_ptr()), "optix_env_shade (backward, ray-record replay)")
-            return (None, None, None, g[0], g[1], None, g[2], g[3], light_grad, None, None, None, None, None, None, None, None, None)
-        # (a device seed tensor must still hold the forward pass's value here: advance it BEFORE the forward call, not after)
-        seed_host, seed_dev = _split_seed(_rnd_seed)
-        L.check(L.lib().mcs_env_shade_bwd(optix_ctx.cpp_wrapper, *[C.byref(x) for x in d], int(ctx.BSDF), int(ctx.n_samples_x),
-                                          seed_host, seed_dev, float(ctx.shadow_scale), int(ctx.batch_offset),
-                                          C.byref(dg), C.byref(sg), g[0].data_ptr(), g[1].data_ptr(), g[2].data_ptr(), g[3].data_ptr(),
-                                          light_grad.data_ptr(), hit.data_ptr() if hit is not None else None, L.stream_ptr()),
-                "optix_env_shade (backward)")
+        else:
+            # (a device seed tensor must still hold the forward pass's value here: advance it BEFORE the forward call, not after)
+            seed_host, seed_dev = _split_seed(_rnd_seed)
+            L.check(L.lib().mcs_env_shade_bwd(optix_ctx.cpp_wrapper, *[C.byref(x) for x in d], int(ctx.BSDF), int(ctx.n_samples_x),
+                                              seed_host, seed_dev, float(ctx.shadow_scale), int(ctx.batch_offset),
+                                              C.byref(dg), C.byref(sg), g[0].data_ptr(), g[1].data_ptr(), g[2].data_ptr(), g[3].data_ptr(),
+                                              light_grad.data_ptr(), hit.data_ptr() if hit is not None else None, L.stream_ptr()),
+                    "optix_env_shade (backward)")
         # same gradient slots as ops.py:105 (no gradient for ro / view_pos / pdf / rows / cols)
         return (None, None, None, g[0], g[1], None, g[2], g[3], light_grad, None, None, None, None, None, None, None, None, None)
 

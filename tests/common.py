@@ -28,10 +28,10 @@ def rel_l2(a, b):
 
 def make_case(res=32, B=1, N=4, mesh="blob+torus", level=2, light="random", light_hw=(32, 64), seed=0, ks_mode="random",
               perm_rows=512, closest=None):
-    """Returns a dict of numpy arrays describing one env_shade problem.
+    """Returns a dict of numpy arrays describing one env_shade problem.  mesh: a synth.scene_mesh kind, or a (verts, tris) pair.
     closest(verts, tris, ro[n,3], rd[n,3]) -> (tri_id[n], tuv[n,3]) overrides the oracle's brute-force primary visibility."""
     o = oracle()
-    v, f = synth.scene_mesh(mesh, level=level, seed=5 + seed)
+    v, f = synth.scene_mesh(mesh, level=level, seed=5 + seed) if isinstance(mesh, str) else mesh
     vn = synth.vertex_normals(v, f)
     scene = o.scene(v, f)
     gbs = []
@@ -96,6 +96,170 @@ def ru_edge_inputs(chans, out_c):
         a[0, 1, 1] = 1e4
     dout = g.uniform(size=shape + (out_c,)).astype(np.float32)
     return ins, dout
+
+
+# ------------------------------------------------------------------------------------------ BVH builds at given triangle counts
+# Triangle counts where the build changes shape (bvh.cu): 1-4 the tiny view, 5-8 an SAH root that may be a leaf run, 1024 the refit's
+# CTA span, 4096 the radix sort's tile, 16 384 the last SAH size, 65 537 seventeen sort tiles.
+BVH_SIZES = [1, 2, 3, 4, 5, 6, 7, 8, 9, 1023, 1024, 1025, 4095, 4096, 4097, 8192, 8193, 16384, 16385, 20481]
+BVH_KINDS = ["coherent", "shuffled", "coincident", "planar"]
+BVH_CASES = [(k, T) for T in BVH_SIZES for k in BVH_KINDS] + [("coincident", 65537)]
+SAH_MAX_TRIS = 16384          # bvh.cu MCS_SAH_MAX_TRIS: 5 <= T <= this get the SAH shadow view
+QSTACK = 100                  # envshade.cu MCS_QSTACK: the shadow-ray walker's stack
+
+
+_SOURCE = {}
+
+
+def _source_mesh(T):
+    """A mesh of at least T triangles: blob level 5 (20 480), or the ~1.08 M-triangle grid above that."""
+    key = "blob5" if T <= 20480 else "grid1m"
+    if key not in _SOURCE:
+        _SOURCE[key] = synth.blob_mesh(5) if key == "blob5" else synth.grid1m_mesh()
+    return _SOURCE[key]
+
+
+def _compact(v, f):
+    used, inv = np.unique(f, return_inverse=True)
+    return np.ascontiguousarray(v[used], np.float32), inv.reshape(f.shape).astype(np.int32)
+
+
+def sized_mesh(kind, T, seed=0):
+    """A mesh of exactly T triangles.
+      coherent:   the first T triangles of a large mesh (input order close to Morton order);
+      shuffled:   a random subset of it in random order, so that every key moves in every sort pass;
+      coincident: a group of distinct triangles inscribed in one box (every axis has one vertex on each face), so they all have the
+                  same box centre and Morton key 0, and their order comes from the sort's stability alone.  For T >= 3 two triangles
+                  come first in the input: one two quantisation cells away in x (key 32: it differs from the group's only in the lowest
+                  radix digit) and one at the far corner of the centroid bounds.  Moving those two shifts the group between passes;
+                  with all keys equal every pass would see the same groups of 32, and four passes that each reversed them would
+                  cancel.  T = 2: the far triangle and one of the group;
+      planar:     cells of a plane at constant y, so the centroid extent in y is 0 (the Morton code's `ext > 0` branch) and the
+                  quantisation grid has only the padding on that axis."""
+    rng = np.random.default_rng(1000 * T + seed)
+    if kind in ("coherent", "shuffled"):
+        v, f = _source_mesh(T)
+        f = f[:T] if kind == "coherent" else f[rng.permutation(f.shape[0])[:T]]
+        return _compact(v, f)
+    if kind == "coincident":
+        lo, hi = np.float32([-0.5, -0.25, -0.75]), np.float32([0.75, 0.5, 0.25])
+        far = np.float32([2.0, 2.0, 2.0])                           # offset of the far triangle's box: the centroid extent
+        shift = np.zeros((T, 3), np.float32)                        # rows 0 .. T - n_group - 1: the two leading triangles
+        if T == 2:
+            shift[0] = far
+        elif T >= 3:
+            shift[0], shift[1] = [2.5 / 1024 * far[0], 0, 0], far
+        r = lo + rng.uniform(0.05, 0.95, (T, 3)) * (hi - lo)
+        a = np.stack([np.full(T, lo[0]), np.full(T, lo[1]), r[:, 2]], -1)
+        b = np.stack([np.full(T, hi[0]), r[:, 1], np.full(T, lo[2])], -1)
+        c = np.stack([r[:, 0], np.full(T, hi[1]), np.full(T, hi[2])], -1)
+        v = (np.stack([a, b, c], 1) + shift[:, None, :]).reshape(-1, 3).astype(np.float32)
+        return v, np.arange(3 * T, dtype=np.int32).reshape(T, 3)
+    if kind == "planar":
+        n = int(np.ceil(np.sqrt(T / 2.0)))
+        v, f = synth.plane_mesh(y=-0.3, half=1.0, n=n)
+        return _compact(v, f[:T])
+    raise ValueError(kind)
+
+
+def bvh_rays(n, seed, v):
+    """Rays from around the mesh towards its centre; one in eight is axis-aligned (zero direction components: slab-test corner cases)."""
+    rng = np.random.default_rng(seed)
+    c = v.mean(0); ext = (v.max(0) - v.min(0)).max()
+    ro = (c + rng.normal(size=(n, 3)) * ext * 0.7).astype(np.float32)
+    tgt = (c + rng.normal(size=(n, 3)) * ext * 0.3).astype(np.float32)
+    rd = tgt - ro
+    rd /= np.linalg.norm(rd, axis=1, keepdims=True)
+    k = n // 8
+    rd[:k] = np.eye(3, dtype=np.float32)[rng.integers(0, 3, k)] * rng.choice([-1.0, 1.0], (k, 1)).astype(np.float32)
+    return ro, rd.astype(np.float32)
+
+
+# ------------------------------------------------------------------------------------------ the shadow-ray view (bvh_export_shadow)
+def walk_shadow_view(ctx):
+    """Walk the exported view from node 0: 4-wide nodes as {node: [child slots]} in walk order (a node after its parent), each used
+    slot ("run", first, count, ql, qh) or ("node", index, None, ql, qh); the triangle ids of the records; the grid; the max depth."""
+    from nvdiffrecmc_b200.optixutils.ops import bvh_export_shadow
+    g = {k: t.cpu().numpy() for k, t in bvh_export_shadow(ctx).items()}
+    nq = g["nodes"].view(np.uint32)
+    ids = g["tris"][:, 0, 3].copy().view(np.int32)
+    nodes, depth, stack = {}, 0, [(0, 1)]
+    while stack:
+        i, d = stack.pop()
+        assert i not in nodes, "node %d reached twice" % i
+        depth = max(depth, d)
+        lb = int(nq[i, 0, 3]) >> 28
+        slots = []
+        for c in range(4):
+            rec = nq[i, c]
+            ql, qh = rec[:3] & 0xFFFF, rec[:3] >> 16
+            if (ql > qh).any():                      # unused slot: inverted box, flagged as a leaf
+                assert (lb >> c) & 1 and (ql == 0xFFFF).all() and (qh == 0).all()
+                continue
+            payload = int(rec[3]) & 0x0FFFFFFF
+            if (lb >> c) & 1:
+                slots.append(("run", payload >> 3, (payload & 7) + 1, ql, qh))
+            else:
+                slots.append(("node", payload, None, ql, qh))
+                stack.append((payload, d + 1))
+        nodes[i] = slots
+    return nodes, ids, g["qgrid"].astype(np.float64), depth
+
+
+def shadow_subtree_bounds(nodes, ids, v, f):
+    """(lo, hi) of the triangles under every node of a walked view, and the per-triangle boxes."""
+    tv = v[f].astype(np.float64)                                     # [T, 3 verts, 3]
+    tlo, thi = tv.min(1), tv.max(1)
+    box = {}
+    for i in reversed(list(nodes)):                                  # children were reached after their parents
+        los, his = [], []
+        for kind, a, n, _, _ in nodes[i]:
+            lo, hi = (tlo[ids[a:a + n]].min(0), thi[ids[a:a + n]].max(0)) if kind == "run" else box[a]
+            los.append(lo); his.append(hi)
+        box[i] = (np.min(los, 0), np.max(his, 0))
+    return box.__getitem__, tlo, thi
+
+
+def shadow_stack_slots(nodes):
+    """Stack entries the walker (envshade.cu:trace_queue) can touch on this view: every hit internal child is pushed and the last one
+    popped at once, so below node v the stack holds sum(internal children - 1) over v's ancestors; a visit stores up to three more."""
+    need, worst = {0: 0}, 0
+    for i, slots in nodes.items():
+        inner = [a for kind, a, _, _, _ in slots if kind == "node"]
+        worst = max(worst, need[i] + 4)
+        for a in inner:
+            need[a] = need[i] + len(inner) - 1
+    return worst
+
+
+def lbvh_collapse_view(ex, T):
+    """The view the walker must find when the shadow rays use the LBVH (T <= 4 or T > SAH_MAX_TRIS): node i holds the grandchildren of
+    binary node i, a subtree of at most four triangles is one run.  {node: [(kind, first or index, count)]}, as walk_shadow_view."""
+    if T <= 4:
+        return {0: [("run", 0, T)]}
+    left, right = ex["left"], ex["right"]
+    span = np.zeros((2 * T - 1, 2), np.int64)
+    span[T - 1:, 0] = span[T - 1:, 1] = np.arange(T)
+    order, stack = [], [0]                  # sorted-triangle range of every internal node, children before parents
+    while stack:
+        i = stack.pop(); order.append(i)
+        stack += [c for c in (left[i], right[i]) if c < T - 1]
+    for i in reversed(order):
+        span[i] = span[left[i], 0], span[right[i], 1]
+
+    def code(c):
+        n = span[c, 1] - span[c, 0] + 1
+        return ("run", int(span[c, 0]), int(n)) if c >= T - 1 or n <= 4 else ("node", int(c), None)
+    view, stack = {}, [0]
+    while stack:
+        i = stack.pop()
+        slots = []
+        for c in (left[i], right[i]):
+            k = code(c)
+            slots += [k] if k[0] == "run" else [code(left[c]), code(right[c])]
+        view[i] = slots
+        stack += [a for kind, a, _ in slots if kind == "node"]
+    return view
 
 
 def env_shade_edge_case():

@@ -5,6 +5,7 @@ import numpy as np
 import pytest
 import torch
 
+from common import bvh_rays as _rays
 from common import oracle
 from nvdiffrecmc_b200 import synth
 
@@ -16,18 +17,6 @@ def _build(dev, v, f):
     ctx = ou.OptiXContext()
     ou.optix_build_bvh(ctx, torch.tensor(v, device=dev), torch.tensor(f, device=dev), rebuild=1)
     return ctx
-
-
-def _rays(n, seed, v):
-    rng = np.random.default_rng(seed)
-    c = v.mean(0); ext = (v.max(0) - v.min(0)).max()
-    ro = (c + rng.normal(size=(n, 3)) * ext * 0.7).astype(np.float32)
-    tgt = (c + rng.normal(size=(n, 3)) * ext * 0.3).astype(np.float32)
-    rd = tgt - ro
-    rd /= np.linalg.norm(rd, axis=1, keepdims=True)
-    k = n // 8            # axis-aligned and zero-component directions (slab-test corner cases)
-    rd[:k] = np.eye(3, dtype=np.float32)[rng.integers(0, 3, k)] * rng.choice([-1.0, 1.0], (k, 1)).astype(np.float32)
-    return ro, rd.astype(np.float32)
 
 
 @pytest.mark.parametrize("kind,level", [("blob", 1), ("blob+torus", 2), ("full", 3)])
@@ -135,7 +124,9 @@ def _assert_structure(dev, v, f):
 
 @pytest.mark.parametrize("kind,level", [("blob+torus", 4), ("bob-like", 4), ("blob+torus", 5)])
 def test_structure_on_both_build_paths(dev, kind, level):
-    """Sizes around the reference's meshes (bob 10 688, spot 5 856 triangles) and one above them.  Both must reproduce the oracle's LBVH bit for bit, and so must the shadow rays that walk it."""
+    """Sizes around the reference's meshes (bob 10 688, spot 5 856 triangles) and one above them.  Both must reproduce the oracle's LBVH bit for
+    bit, and the visibility queries on its fp32 nodes must equal the oracle's LBVH traversal.  (The shadow rays walk a separate view:
+    tests/test_gpu_shadow_bvh.py and tests/test_gpu_bvh_sizes.py.)"""
     v, f = synth.scene_mesh(kind, level=level)
     ctx = _assert_structure(dev, v, f)
     import nvdiffrecmc_b200.optixutils as ou

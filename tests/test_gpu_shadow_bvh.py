@@ -5,11 +5,12 @@ import numpy as np
 import pytest
 import torch
 
-from common import oracle
+from common import QSTACK, oracle
+from common import shadow_subtree_bounds as _subtree_bounds
+from common import walk_shadow_view as _walk
 from nvdiffrecmc_b200 import synth
 
 pytestmark = pytest.mark.gpu
-QSTACK = 100          # envshade.cu MCS_QSTACK: up to 3 pushes per 4-wide level + one scratch slot
 
 
 def _build(dev, v, f, rebuild_from=None):
@@ -19,52 +20,6 @@ def _build(dev, v, f, rebuild_from=None):
     if rebuild_from is not None:
         ou.optix_build_bvh(ctx, torch.tensor(v, device=dev), torch.tensor(f, device=dev), rebuild=0)
     return ctx
-
-
-def _walk(ctx):
-    """Walk the exported view from node 0: 4-wide nodes as (node, [child slots]), leaf runs as (first, count), max depth."""
-    from nvdiffrecmc_b200.optixutils.ops import bvh_export_shadow
-    g = {k: t.cpu().numpy() for k, t in bvh_export_shadow(ctx).items()}
-    nq = g["nodes"].view(np.uint32)
-    ids = g["tris"][:, 0, 3].copy().view(np.int32)
-    nodes, depth, stack = {}, 0, [(0, 1)]
-    while stack:
-        i, d = stack.pop()
-        assert i not in nodes, "node %d reached twice" % i
-        depth = max(depth, d)
-        lb = int(nq[i, 0, 3]) >> 28
-        slots = []
-        for c in range(4):
-            rec = nq[i, c]
-            ql, qh = rec[:3] & 0xFFFF, rec[:3] >> 16
-            if (ql > qh).any():                      # unused slot: inverted box, flagged as a leaf
-                assert (lb >> c) & 1 and (ql == 0xFFFF).all() and (qh == 0).all()
-                continue
-            payload = int(rec[3]) & 0x0FFFFFFF
-            if (lb >> c) & 1:
-                slots.append(("run", payload >> 3, (payload & 7) + 1, ql, qh))
-            else:
-                slots.append(("node", payload, None, ql, qh))
-                stack.append((payload, d + 1))
-        nodes[i] = slots
-    return nodes, ids, g["qgrid"].astype(np.float64), depth
-
-
-def _subtree_bounds(nodes, ids, v, f):
-    """(lo, hi) of the triangles under every slot, and the set of triangle slots covered by each run."""
-    tv = v[f].astype(np.float64)                                     # [T, 3 verts, 3]
-    tlo, thi = tv.min(1), tv.max(1)
-    memo = {}
-
-    def node_bounds(i):
-        if i not in memo:
-            los, his = [], []
-            for kind, a, n, _, _ in nodes[i]:
-                lo, hi = (tlo[ids[a:a + n]].min(0), thi[ids[a:a + n]].max(0)) if kind == "run" else node_bounds(a)
-                los.append(lo); his.append(hi)
-            memo[i] = (np.min(los, 0), np.max(his, 0))
-        return memo[i]
-    return node_bounds, tlo, thi
 
 
 CASES = [("blob", 1), ("blob+torus", 4), ("bob-like", 4)]

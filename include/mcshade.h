@@ -264,6 +264,24 @@ int mcs_texel_fetch_bwd(int64_t T, int32_t C, const int64_t *idx, int64_t n, con
  *      (holds the un-normalised row sums on return).  Sums are carried in fp64 and rounded once. */
 int mcs_update_pdf(const mcs_tensor *base, float *pdf, float *rows, float *cols, double *row_totals, mcs_stream s);
 
+/* ---- multiresolution hash-grid encoding: stands in for tiny-cuda-nn's `HashGrid` Encoding behind MLPTexture3D (render/mlptexture.py:57-73),
+ *      3 input dimensions, 2 features per level, linear interpolation; semantics in csrc/hashgrid.cu.
+ *      The level table is built on the host (nvdiffrecmc_b200/tinycudann) and passed by value: offset[l] is the first entry of level l
+ *      (offset[n_levels] = total entries; non-decreasing multiples of 8, every level non-empty), res / scale its resolution and scale,
+ *      bit l of dense_mask set for a dense level.  x [n,3], out / d_out [n, 2*n_levels], params / d_params [2 * offset[n_levels]], d_x [n,3]:
+ *      fp32, contiguous; params, out, d_out, d_params 8-byte aligned.  The backward adds into d_params (caller-zeroed, float atomics; may be
+ *      null) and overwrites d_x (deterministic; may be null; not both null).  n = 0 is a no-op.  No host sync, no allocation. */
+typedef struct mcs_hashgrid_levels {
+    int32_t n_levels;
+    uint32_t offset[17];
+    uint32_t res[16];
+    float scale[16];
+    uint32_t dense_mask;
+} mcs_hashgrid_levels;
+int mcs_hashgrid_fwd(const float *x, int64_t n, const float *params, const mcs_hashgrid_levels *lv, float *out, mcs_stream stream);
+int mcs_hashgrid_bwd(const float *x, int64_t n, const float *params, const mcs_hashgrid_levels *lv, const float *d_out, float *d_params,
+                     float *d_x, mcs_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,7 +14,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_PKG, "csrc")
 _LIBDIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
-SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu"]
+SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
@@ -59,6 +59,10 @@ def build(force=False, verbose=False):
         if verbose:
             print("[mcshade] linked", LIB_PATH)
     return LIB_PATH
+
+
+class mcs_hashgrid_levels(C.Structure):
+    _fields_ = [("n_levels", C.c_int32), ("offset", C.c_uint32 * 17), ("res", C.c_uint32 * 16), ("scale", C.c_float * 16), ("dense_mask", C.c_uint32)]
 
 
 class mcs_tensor(C.Structure):
@@ -125,6 +129,8 @@ _SIGS = {
     "mcs_aa_topology": ([_P, C.c_int32, _P, _P, _P], C.c_int),
     "mcs_antialias_fwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P], C.c_int),
     "mcs_antialias_bwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
+    "mcs_hashgrid_fwd": ([_P, C.c_int64, _P, _P, _P, _P], C.c_int),
+    "mcs_hashgrid_bwd": ([_P, C.c_int64, _P, _P, _P, _P, _P, _P], C.c_int),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 
@@ -154,7 +160,7 @@ def lib():
 # and for meshes of 5 to 16 384 triangles the shadow view's clustering and emission.
 LAUNCHES = collections.Counter()
 _KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "rasterize_peel": 2,
-                     "antialias_topology": 2}
+                     "antialias_topology": 2, "hashgrid_bwd_both": 2}
 
 
 def check(status, what):

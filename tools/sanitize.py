@@ -62,6 +62,12 @@ with DepthPeeler(ctx, mg, (24, 24), posp, t("tris")) as peeler:
     layers = [peeler.rasterize_next_layer()[0] for _ in range(3)]
 sum(antialias(rl[..., 3:4].clamp(0, 1), rl, posp, t("tris")).sum() + rl[..., :2].sum() for rl in layers).backward()
 ou.trace_closest(ctx, t("ro").reshape(-1, 3), torch.randn(c["ro"].size // 3, 3, device=dev), t_after=torch.rand(c["ro"].size // 3, device=dev))
+# hash-grid encoding: forward, d params + d x, d params only, on a padded dense level, an exact-fit level and hashed levels
+from nvdiffrecmc_b200.tinycudann import Encoding
+enc = Encoding(3, {"otype": "HashGrid", "n_levels": 5, "log2_hashmap_size": 9, "base_resolution": 5, "per_level_scale": 1.5})
+xh = (torch.rand(1000, 3, device=dev) * 2 - 0.5).requires_grad_(True)
+enc(xh).sum().backward()
+enc(xh.detach()).sum().backward()
 if os.environ.get("MCS_EW_TMA"):
     B, H, W = 1, 400, 400          # 160 000 px = 312 tiles of 512 px (>= 2 x 132) + a ragged tail
     ins = [torch.rand(B, H, W, 3, device=dev).requires_grad_(True) for _ in range(6)]

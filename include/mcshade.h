@@ -246,6 +246,26 @@ int mcs_rasterize_bwd(const float *pos, int64_t pos_batch_stride, int32_t V, con
                       int32_t W, const float *d_rast, float *d_pos, mcs_stream stream);
 int mcs_interpolate_bwd_rast(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
                              int32_t B, int32_t H, int32_t W, const float *d_out, float *d_attr, float *d_rast, mcs_stream stream);
+
+/* ---- screen-space derivatives (render/render.py:225-234: dr.interpolate(..., rast_db=, diff_attrs='all') builds gb_texc_deriv and the
+ *      denoiser's depth guide gb_depth); semantics in csrc/raster.cu.  pos / tris / rast as mcs_rasterize_bwd.
+ *   rast_db: rast_db [B,H,W,4] = (du/dX, du/dY, dv/dX, dv/dY) in pixels (nvdiffrast's layout) for the triangle id stored in rast, from pos
+ *      alone; 0 for background, ids >= T and degenerate (S == 0) pixels.  Bit-reproducible (explicitly rounded).
+ *   rasterize_bwd_db: d_rast (may be null) and d_rast_db [B,H,W,4] -> d_pos (caller-zeroed, float atomics).
+ *   interpolate_da: out_da [B,H,W,2*n_diff], channels 2k / 2k+1 = (dA/dX, dA/dY) of the k-th selected attribute; diff_idx is a HOST array of
+ *      n_diff (1..32) indices in [0, C), repeats allowed, or NULL for all C attributes in order (then n_diff must equal C).  The backward
+ *      adds into d_attr (caller-zeroed, float atomics; may be null) and overwrites d_rast_db [B,H,W,4] (may be null; not both null). */
+int mcs_rast_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B, int32_t H,
+                int32_t W, float *rast_db, mcs_stream stream);
+int mcs_rasterize_bwd_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B,
+                         int32_t H, int32_t W, const float *d_rast, const float *d_rast_db, float *d_pos, mcs_stream stream);
+int mcs_interpolate_da_fwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
+                           const float *rast_db, int32_t B, int32_t H, int32_t W, int32_t n_diff, const int32_t *diff_idx, float *out_da,
+                           mcs_stream stream);
+int mcs_interpolate_da_bwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
+                           const float *rast_db, int32_t B, int32_t H, int32_t W, int32_t n_diff, const int32_t *diff_idx, const float *d_out_da,
+                           float *d_attr, float *d_rast_db, mcs_stream stream);
+
 int64_t mcs_aa_topology_workspace_bytes(int32_t T);
 int mcs_aa_topology(const int32_t *tris, int32_t T, void *workspace, int32_t *adj, mcs_stream stream);
 int mcs_antialias_fwd(const float *color, int32_t C, const float *rast, int32_t B, int32_t H, int32_t W, const float *pos, int64_t pos_batch_stride,

@@ -125,6 +125,12 @@ _SIGS = {
     "mcs_interpolate_bwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
     "mcs_interpolate_bwd_rast": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P], C.c_int),
     "mcs_rasterize_bwd": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
+    "mcs_rast_db": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
+    "mcs_rasterize_bwd_db": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P], C.c_int),
+    "mcs_interpolate_da_fwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P],
+                               C.c_int),
+    "mcs_interpolate_da_bwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
+                                _P, _P], C.c_int),
     "mcs_aa_topology_workspace_bytes": ([C.c_int32], C.c_int64),
     "mcs_aa_topology": ([_P, C.c_int32, _P, _P, _P], C.c_int),
     "mcs_antialias_fwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P], C.c_int),

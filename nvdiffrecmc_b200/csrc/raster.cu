@@ -31,6 +31,27 @@
 //                       d x_k = dL/da_k.x,  d y_k = dL/da_k.y,  d w_k = -px dL/da_k.x - py dL/da_k.y.
 //                     z/w and the id carry no gradient (the reference computes depth under no_grad, render.py:228-234).
 //                     One thread per pixel; warp-aggregated float atomics (see the kernel).
+//
+// Screen-space derivatives (render/render.py:225-234 builds the denoiser's depth guide from them; nvdiffrast's layout):
+//
+//   k_rast_db       : rast_db[b,y,x] = (du/dX, du/dY, dv/dX, dv/dY), X the column and Y the row index in pixels, for the triangle id
+//                     stored in rast, from the clip-space pos alone.  With the terms above the px py products cancel, so every s_i is
+//                     affine in (px, py):
+//                       ds_i/dpx = y_{i+1} w_{i+2} - w_{i+1} y_{i+2},   ds_i/dpy = w_{i+1} x_{i+2} - x_{i+1} w_{i+2},
+//                       du/dpx = (ds0/dpx - u dS/dpx) / S  (likewise py, and v with s1),   d/dX = (2/W) d/dpx,  d/dY = (2/H) d/dpy.
+//                     All four channels are 0 for background, ids >= T and S == 0.  Every operation is explicitly rounded in one fixed
+//                     order (the fp32 build of oracle/raster_db.c evaluates the same order), so rast_db is bit-reproducible.  A vertex
+//                     with w <= 0 needs no special case: the projective formula holds wherever the pixel has a hit.  One launch after
+//                     rasterize or any peel layer; k_rasterize is unchanged.
+//   k_interpolate_da: out_da[b,y,x,2k:2k+2] = (dA/dX, dA/dY) of the k-th selected attribute A (attribute-major, nvdiffrast's layout):
+//                       dA/dX = db.x (A0 - A2) + db.z (A1 - A2),   dA/dY = db.y (A0 - A2) + db.w (A1 - A2),   0 without a hit.
+//                     The selection ('all' or up to 32 indices, repeats allowed) is passed by value.  out_da does not depend on u, v.
+//                     Backward: d attr by float atomics (dA0 += gX db.x + gY db.y, dA1 += gX db.z + gY db.w, dA2 -= both), and
+//                     d rast_db = (sum gX (A0 - A2), sum gY (A0 - A2), sum gX (A1 - A2), sum gY (A1 - A2)) over the selection, one writer
+//                     per pixel in the selection's order (bit-reproducible).
+//   k_rasterize_bwd<true>: d rast[...,0:2] (optional) and d rast_db -> d pos.  The rast_db term differentiates the formula above with
+//                     respect to s_i, S and the ds_i/dp terms, then maps dL/ds_i to d pos like the barycentric term and adds the direct
+//                     terms of ds_i/dp in (x_k, y_k, w_k).  k_rasterize_bwd<false> is the d rast-only kernel.
 //   k_aa_topo_*     : edge adjacency of a triangle list: the 3T undirected edge keys go into an open-addressing hash table (64-bit
 //                     atomicCAS, linear probing) that counts the triangles on each key and keeps the first two; a second pass resolves
 //                     adj[t,k] = the other triangle on edge (tri[t,k], tri[t,(k+1)%3]), -1 on a boundary edge, -2 with three or more.
@@ -176,6 +197,95 @@ __global__ void __launch_bounds__(256) k_interpolate(const InterpParams p)
     if (MODE == 2) p.drast[i] = make_float4(du, dv, 0.0f, 0.0f);
 }
 
+#define MCS_DIFF_ATTRS_MAX 32
+
+struct InterpDaParams {
+    const float *attr; int64_t attr_bs; int V, C;
+    const int32_t *tris; int T;
+    const float4 *rast, *db;
+    float *out_da;                              // forward: [B,H,W,2n]
+    const float *dout_da; float *dattr;         // backward: d out_da [B,H,W,2n]; d attr (caller-zeroed, atomics) or null
+    float4 *ddb;                                // backward: d rast_db (every pixel written) or null
+    int64_t npx, px_per_batch;
+    int n, all;                                 // n selected attributes; all != 0: the k-th is attribute k, else idx[k]
+    int32_t idx[MCS_DIFF_ATTRS_MAX];
+};
+
+// out_da and its backward (semantics in the file header).  Differences and products are explicitly rounded so the forward and
+// d rast_db equal the fp32 oracle bit for bit.
+// d attr: with MCS_DA_AGG, lanes of a warp that hit the same triangle of the same image sum their per-vertex terms with shuffles
+// (__match_any_sync groups, as k_rasterize_bwd) and one lane issues the atomics.
+#ifndef MCS_DA_AGG
+#define MCS_DA_AGG 1
+#endif
+template <bool BWD>
+__global__ void __launch_bounds__(256) k_interpolate_da(const InterpDaParams p)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool agg = BWD && MCS_DA_AGG && p.dattr;      // then every lane of the warp reaches __match_any_sync (no early exit before it)
+    if (i >= p.npx && !agg) return;
+    int id = -1;
+    if (i < p.npx) {
+        id = (int)__ldg(p.rast + i).w - 1;
+        if (id >= p.T) id = -1;
+    }
+    const int n = p.n;
+    if (id < 0 && i < p.npx) {
+        if (!BWD) for (int k = 0; k < 2 * n; ++k) p.out_da[i * 2 * n + k] = 0.0f;
+        if (BWD && p.ddb) p.ddb[i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+    const unsigned lane = threadIdx.x & 31u;
+    unsigned peers = 1u << lane;
+    if (agg) {
+        const long long key = id >= 0 ? (long long)(i / p.px_per_batch) * p.T + id : -1ll - (long long)lane;
+        peers = __match_any_sync(0xFFFFFFFFu, key);
+    }
+    if (id < 0) return;
+    const int i0 = __ldg(p.tris + 3 * (size_t)id), i1 = __ldg(p.tris + 3 * (size_t)id + 1), i2 = __ldg(p.tris + 3 * (size_t)id + 2);
+    const int64_t base = (i / p.px_per_batch) * p.attr_bs;
+    const float4 db = __ldg(p.db + i);
+    const bool need_a = !BWD || p.ddb;
+    float e0 = 0.0f, e1 = 0.0f, e2 = 0.0f, e3 = 0.0f;
+    for (int k = 0; k < n; ++k) {
+        const int c = p.all ? k : p.idx[k];
+        float d0 = 0.0f, d1 = 0.0f;
+        if (need_a) {
+            const float *A = p.attr + base;
+            const float a2 = __ldg(A + (size_t)i2 * p.C + c);
+            d0 = __fsub_rn(__ldg(A + (size_t)i0 * p.C + c), a2);
+            d1 = __fsub_rn(__ldg(A + (size_t)i1 * p.C + c), a2);
+        }
+        if (!BWD) {
+            p.out_da[(i * n + k) * 2] = __fadd_rn(__fmul_rn(db.x, d0), __fmul_rn(db.z, d1));
+            p.out_da[(i * n + k) * 2 + 1] = __fadd_rn(__fmul_rn(db.y, d0), __fmul_rn(db.w, d1));
+        } else {
+            const float gX = __ldg(p.dout_da + (i * n + k) * 2), gY = __ldg(p.dout_da + (i * n + k) * 2 + 1);
+            if (p.dattr) {
+                float a0 = gX * db.x + gY * db.y, a1 = gX * db.z + gY * db.w;
+                bool issue = gX != 0.0f || gY != 0.0f;
+                if (agg && peers != (1u << lane)) {
+                    float s0 = 0.0f, s1 = 0.0f;
+                    for (unsigned m = peers; m; m &= m - 1) {
+                        const int src = __ffs(m) - 1;
+                        s0 += __shfl_sync(peers, a0, src); s1 += __shfl_sync(peers, a1, src);
+                    }
+                    a0 = s0; a1 = s1;
+                    issue = (int)lane == __ffs(peers) - 1 && (a0 != 0.0f || a1 != 0.0f);
+                }
+                if (issue) {
+                    float *D = p.dattr + base;
+                    atomicAdd(D + (size_t)i0 * p.C + c, a0); atomicAdd(D + (size_t)i1 * p.C + c, a1); atomicAdd(D + (size_t)i2 * p.C + c, -(a0 + a1));
+                }
+            }
+            if (p.ddb) {
+                e0 = __fadd_rn(e0, __fmul_rn(gX, d0)); e1 = __fadd_rn(e1, __fmul_rn(gY, d0));
+                e2 = __fadd_rn(e2, __fmul_rn(gX, d1)); e3 = __fadd_rn(e3, __fmul_rn(gY, d1));
+            }
+        }
+    }
+    if (BWD && p.ddb) p.ddb[i] = make_float4(e0, e1, e2, e3);
+}
+
 // ------------------------------------------------------------------------------------------------------------------------------------
 // rasterize backward: d rast[...,0:2] -> d pos through u = s0 / S, v = s1 / S (derivation in the file header)
 // ------------------------------------------------------------------------------------------------------------------------------------
@@ -185,14 +295,62 @@ struct RastBwdParams {
     const float4 *rast, *drast;
     int B, H, W;
     float *dpos;
+    const float4 *drast_db;      // k_rasterize_bwd<true>: d rast_db (drast may then be null)
+    float4 *rast_db;             // k_rast_db: output
 };
 
 // NDC coordinate of pixel centre i of n (image row iy -> NDC y = (iy + 0.5) / H * 2 - 1, as k_rasterize), explicitly rounded
 __device__ __forceinline__ float px_ndc(int i, int n) { return __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn((float)i, 0.5f), (float)n), 2.0f), 1.0f); }
 
+// rast_db (file header): one thread per pixel, explicitly rounded in the order of oracle/raster_db.c's orc_rast_db
+__global__ void __launch_bounds__(256) k_rast_db(const RastBwdParams p)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t n = (int64_t)p.B * p.H * p.W;
+    if (i >= n) return;
+    const float4 r = __ldg(p.rast + i);
+    const int id = (int)r.w - 1;
+    float4 out = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    if (id >= 0 && id < p.T) {
+        const int ix = (int)(i % p.W); const int64_t t_ = i / p.W; const int iy = (int)(t_ % p.H), b = (int)(t_ / p.H);
+        const float px = px_ndc(ix, p.W), py = px_ndc(iy, p.H);
+        const float *P = p.pos + (int64_t)b * p.pos_bs;
+        float x[3], y[3], w[3], ax[3], ay[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const float *q = P + 4 * (size_t)__ldg(p.tris + 3 * (size_t)id + k);
+            x[k] = __ldg(q); y[k] = __ldg(q + 1); w[k] = __ldg(q + 3);
+            ax[k] = __fsub_rn(x[k], __fmul_rn(px, w[k])); ay[k] = __fsub_rn(y[k], __fmul_rn(py, w[k]));
+        }
+        const float s0 = __fsub_rn(__fmul_rn(ax[1], ay[2]), __fmul_rn(ay[1], ax[2]));
+        const float s1 = __fsub_rn(__fmul_rn(ax[2], ay[0]), __fmul_rn(ay[2], ax[0]));
+        const float s2 = __fsub_rn(__fmul_rn(ax[0], ay[1]), __fmul_rn(ay[0], ax[1]));
+        const float S = __fadd_rn(__fadd_rn(s0, s1), s2);
+        if (S != 0.0f) {
+            float dx[3], dy[3];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const int k1 = k == 2 ? 0 : k + 1, k2 = k == 0 ? 2 : k - 1;
+                dx[k] = __fsub_rn(__fmul_rn(y[k1], w[k2]), __fmul_rn(w[k1], y[k2]));
+                dy[k] = __fsub_rn(__fmul_rn(w[k1], x[k2]), __fmul_rn(x[k1], w[k2]));
+            }
+            const float dSx = __fadd_rn(__fadd_rn(dx[0], dx[1]), dx[2]), dSy = __fadd_rn(__fadd_rn(dy[0], dy[1]), dy[2]);
+            const float u = __fdiv_rn(s0, S), v = __fdiv_rn(s1, S);
+            const float sx = __fdiv_rn(2.0f, (float)p.W), sy = __fdiv_rn(2.0f, (float)p.H);
+            out.x = __fmul_rn(__fdiv_rn(__fsub_rn(dx[0], __fmul_rn(u, dSx)), S), sx);
+            out.y = __fmul_rn(__fdiv_rn(__fsub_rn(dy[0], __fmul_rn(u, dSy)), S), sy);
+            out.z = __fmul_rn(__fdiv_rn(__fsub_rn(dx[1], __fmul_rn(v, dSx)), S), sx);
+            out.w = __fmul_rn(__fdiv_rn(__fsub_rn(dy[1], __fmul_rn(v, dSy)), S), sy);
+        }
+    }
+    p.rast_db[i] = out;
+}
+
 // Lanes of a warp that hit the same triangle of the same image sum their 9 vertex gradients with shuffles (__match_any_sync groups,
 // summed in lane order) and one lane issues the atomics: 0.093 ms against 0.354 ms with 9 atomics per pixel at 8 x 512^2 on the bench
 // mesh (H100 80GB HBM3, 400 W), where consecutive pixels of a row mostly share a triangle.
+// DB: d rast (may be null) and d rast_db; without DB this is the d rast-only kernel.
+template <bool DB>
 __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -203,19 +361,26 @@ __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
     if (i < n) {
         const float4 r = __ldg(p.rast + i);
         id = (int)r.w - 1;
-        const float4 g = __ldg(p.drast + i);
-        if (id >= p.T || (g.x == 0.0f && g.y == 0.0f)) id = -1;
+        const float4 g = DB && !p.drast ? make_float4(0.0f, 0.0f, 0.0f, 0.0f) : __ldg(p.drast + i);
+        float4 h = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        bool zero = g.x == 0.0f && g.y == 0.0f;
+        if (DB) {
+            h = __ldg(p.drast_db + i);
+            zero = zero && h.x == 0.0f && h.y == 0.0f && h.z == 0.0f && h.w == 0.0f;
+        }
+        if (id >= p.T || zero) id = -1;
         if (id >= 0) {
             const int ix = (int)(i % p.W); const int64_t t_ = i / p.W; const int iy = (int)(t_ % p.H); b = (int)(t_ / p.H);
             const float px = px_ndc(ix, p.W), py = px_ndc(iy, p.H);
             const float *P = p.pos + (int64_t)b * p.pos_bs;
-            float ax[3], ay[3];
+            float ax[3], ay[3], x[3], y[3], wv[3];
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 vi[k] = __ldg(p.tris + 3 * (size_t)id + k);
                 const float *q = P + 4 * (size_t)vi[k];
                 const float w = __ldg(q + 3);
                 ax[k] = __fsub_rn(__ldg(q), __fmul_rn(px, w)); ay[k] = __fsub_rn(__ldg(q + 1), __fmul_rn(py, w));
+                if (DB) { x[k] = __ldg(q); y[k] = __ldg(q + 1); wv[k] = w; }
             }
             const float s0 = __fsub_rn(__fmul_rn(ax[1], ay[2]), __fmul_rn(ay[1], ax[2]));
             const float s1 = __fsub_rn(__fmul_rn(ax[2], ay[0]), __fmul_rn(ay[2], ax[0]));
@@ -225,13 +390,39 @@ __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
                 id = -1;
             } else {
                 const float u = s0 / S, v = s1 / S, G = g.x * u + g.y * v;
-                const float gs[3] = {(g.x - G) / S, (g.y - G) / S, -G / S};
+                float gs[3] = {(g.x - G) / S, (g.y - G) / S, -G / S};
+                float ex[3], ey[3];
+                if (DB) {
+                    // L = sum_{c = u, v; p = px, py} h_cp (ds_c/dp - c dS/dp) / S with h the pixel-scaled d rast_db
+                    float dx[3], dy[3];
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        const int k1 = k == 2 ? 0 : k + 1, k2 = k == 0 ? 2 : k - 1;
+                        dx[k] = y[k1] * wv[k2] - wv[k1] * y[k2];
+                        dy[k] = wv[k1] * x[k2] - x[k1] * wv[k2];
+                    }
+                    const float dSx = dx[0] + dx[1] + dx[2], dSy = dy[0] + dy[1] + dy[2];
+                    const float sx = 2.0f / (float)p.W, sy = 2.0f / (float)p.H;
+                    const float hxu = h.x * sx, hyu = h.y * sy, hxv = h.z * sx, hyv = h.w * sy;
+                    const float Kx = hxu * u + hxv * v, Ky = hyu * u + hyv * v;
+                    ex[0] = (hxu - Kx) / S; ex[1] = (hxv - Kx) / S; ex[2] = -Kx / S;          // dL / d(ds_i/dpx)
+                    ey[0] = (hyu - Ky) / S; ey[1] = (hyv - Ky) / S; ey[2] = -Ky / S;          // dL / d(ds_i/dpy)
+                    const float mu = -(hxu * dSx + hyu * dSy) / S, mv = -(hxv * dSx + hyv * dSy) / S;      // dL/du, dL/dv
+                    const float Ldb = (hxu * (dx[0] - u * dSx) + hyu * (dy[0] - u * dSy) + hxv * (dx[1] - v * dSx) + hyv * (dy[1] - v * dSy)) / S;
+                    const float GS = -(Ldb + mu * u + mv * v) / S;                                  // dL/dS
+                    gs[0] += mu / S + GS; gs[1] += mv / S + GS; gs[2] += GS;
+                }
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
                     const int k1 = k == 2 ? 0 : k + 1, k2 = k == 0 ? 2 : k - 1;
                     gx[k] = gs[k2] * ay[k1] - gs[k1] * ay[k2];
                     gy[k] = gs[k1] * ax[k2] - gs[k2] * ax[k1];
                     gw[k] = -px * gx[k] - py * gy[k];
+                    if (DB) {
+                        gx[k] += ey[k1] * wv[k2] - ey[k2] * wv[k1];
+                        gy[k] += ex[k2] * wv[k1] - ex[k1] * wv[k2];
+                        gw[k] += ex[k1] * y[k2] - ex[k2] * y[k1] + ey[k2] * x[k1] - ey[k1] * x[k2];
+                    }
                 }
             }
         }
@@ -595,7 +786,84 @@ int mcs_rasterize_bwd(const float *pos, int64_t pos_batch_stride, int32_t V, con
     p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast; p.drast = (const float4 *)d_rast;
     p.B = B; p.H = H; p.W = W; p.dpos = d_pos;
     const int64_t n = (int64_t)B * H * W;
-    k_rasterize_bwd<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
+    k_rasterize_bwd<false><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_rast_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B, int32_t H,
+                int32_t W, float *rast_db, mcs_stream stream)
+{
+    MCS_REQUIRE(pos && tris && rast && rast_db && V > 0 && T > 0 && B > 0 && H > 0 && W > 0 && pos_batch_stride >= 0, "mcs_rast_db: bad arguments");
+    RastBwdParams p{};
+    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast;
+    p.B = B; p.H = H; p.W = W; p.rast_db = (float4 *)rast_db;
+    const int64_t n = (int64_t)B * H * W;
+    k_rast_db<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_rasterize_bwd_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B,
+                         int32_t H, int32_t W, const float *d_rast, const float *d_rast_db, float *d_pos, mcs_stream stream)
+{
+    MCS_REQUIRE(pos && tris && rast && d_rast_db && d_pos && V > 0 && T > 0 && B > 0 && H > 0 && W > 0 && pos_batch_stride >= 0,
+                "mcs_rasterize_bwd_db: bad arguments");
+    RastBwdParams p{};
+    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast; p.drast = (const float4 *)d_rast;
+    p.drast_db = (const float4 *)d_rast_db; p.B = B; p.H = H; p.W = W; p.dpos = d_pos;
+    const int64_t n = (int64_t)B * H * W;
+    k_rasterize_bwd<true><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+static int interp_da_common(InterpDaParams &p, const char *name, const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C,
+                            const int32_t *tris, int32_t T, const float *rast, const float *rast_db, int32_t B, int32_t H, int32_t W,
+                            int32_t n_diff, const int32_t *diff_idx)
+{
+    MCS_REQUIRE(attr && tris && rast && rast_db && V > 0 && C > 0 && T > 0 && B > 0 && H > 0 && W > 0 && attr_batch_stride >= 0,
+                "%s: bad arguments", name);
+    if (diff_idx == nullptr) {
+        MCS_REQUIRE(n_diff == C, "%s: without an index list n_diff (%d) must equal C (%d)", name, n_diff, C);
+    } else {
+        MCS_REQUIRE(n_diff >= 1 && n_diff <= MCS_DIFF_ATTRS_MAX, "%s: %d attribute indices (1 to %d allowed)", name, n_diff, MCS_DIFF_ATTRS_MAX);
+        for (int k = 0; k < n_diff; ++k) {
+            MCS_REQUIRE(diff_idx[k] >= 0 && diff_idx[k] < C, "%s: attribute index %d out of range [0, %d)", name, diff_idx[k], C);
+            p.idx[k] = diff_idx[k];
+        }
+    }
+    p.attr = attr; p.attr_bs = attr_batch_stride; p.V = V; p.C = C; p.tris = tris; p.T = T;
+    p.rast = (const float4 *)rast; p.db = (const float4 *)rast_db;
+    p.px_per_batch = (int64_t)H * W; p.npx = p.px_per_batch * B;
+    p.n = n_diff; p.all = diff_idx == nullptr;
+    return 0;
+}
+
+int mcs_interpolate_da_fwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
+                           const float *rast_db, int32_t B, int32_t H, int32_t W, int32_t n_diff, const int32_t *diff_idx, float *out_da,
+                           mcs_stream stream)
+{
+    InterpDaParams p{};
+    if (int e = interp_da_common(p, "mcs_interpolate_da_fwd", attr, attr_batch_stride, V, C, tris, T, rast, rast_db, B, H, W, n_diff, diff_idx))
+        return e;
+    MCS_REQUIRE(out_da != nullptr, "mcs_interpolate_da_fwd: null output");
+    p.out_da = out_da;
+    k_interpolate_da<false><<<(unsigned)((p.npx + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_interpolate_da_bwd(const float *attr, int64_t attr_batch_stride, int32_t V, int32_t C, const int32_t *tris, int32_t T, const float *rast,
+                           const float *rast_db, int32_t B, int32_t H, int32_t W, int32_t n_diff, const int32_t *diff_idx, const float *d_out_da,
+                           float *d_attr, float *d_rast_db, mcs_stream stream)
+{
+    InterpDaParams p{};
+    if (int e = interp_da_common(p, "mcs_interpolate_da_bwd", attr, attr_batch_stride, V, C, tris, T, rast, rast_db, B, H, W, n_diff, diff_idx))
+        return e;
+    MCS_REQUIRE(d_out_da && (d_attr || d_rast_db), "mcs_interpolate_da_bwd: null gradient pointer");
+    p.dout_da = d_out_da; p.dattr = d_attr; p.ddb = (float4 *)d_rast_db;
+    k_interpolate_da<true><<<(unsigned)((p.npx + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
     MCS_LAUNCH_CHECK();
     return 0;
 }

@@ -8,7 +8,12 @@ those barycentrics and is differentiable with respect to the attributes and to `
 antialiasing of Laine et al. 2020, the only path from coverage (alpha) to vertex positions, so silhouette losses train the mesh;
 `antialias_topology` builds the edge adjacency it needs on the device.  `DepthPeeler` returns the deeper layers of the same G-buffer
 (the next surface along each primary ray), each an ordinary `rast` that `interpolate` and `antialias` take, as render_mesh's
-back-to-front `composite_buffer` needs.  Screen-space derivatives (`rast_db`, `diff_attrs`) are not provided."""
+back-to-front `composite_buffer` needs.  Screen-space derivatives come in nvdiffrast's layout: `rasterize(grad_db=True)` and
+`DepthPeeler(grad_db=True)` also return `rast_db` (du/dX, du/dY, dv/dX, dv/dY in pixels, from the clip-space triangle), and
+`interpolate(..., rast_db=, diff_attrs=)` returns the attribute derivatives `out_da` that render_layer turns into the denoiser's depth
+guide (render.py:225-234)."""
+import ctypes
+
 import torch
 from . import _lib as L
 
@@ -61,6 +66,48 @@ class _rasterize_func(torch.autograd.Function):
         return d_pos, None, None, None, None, None
 
 
+def _pos_args(pos):
+    V = pos.shape[-2]
+    return pos.data_ptr(), V * 4 if pos.dim() == 3 else 0, V
+
+
+def _rast_db_launch(pos, tri, rast):
+    """rast_db [B,H,W,4] of `rast` from the clip-space pos (contiguous fp32) and tri (contiguous int32); no autograd."""
+    B, H, W = rast.shape[0], rast.shape[1], rast.shape[2]
+    db = torch.empty(B, H, W, 4, dtype=torch.float32, device=rast.device)
+    L.check(L.lib().mcs_rast_db(*_pos_args(pos), tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W, db.data_ptr(), L.stream_ptr()), "rast_db")
+    return db
+
+
+class _rasterize_db_func(torch.autograd.Function):
+    """(rast, rast_db) of one rasterize or peel launch; the backward maps d rast and d rast_db to d pos in one launch."""
+    @staticmethod
+    def forward(ctx, pos, tri, optix_ctx, m, resolution, t_state=None):
+        ctx.set_materialize_grads(False)
+        rast = _rasterize_launch(optix_ctx, m, resolution, t_state)
+        db = _rast_db_launch(pos, tri, rast)
+        ctx.save_for_backward(pos, tri, rast)
+        return rast, db
+
+    @staticmethod
+    def backward(ctx, d_rast, d_db):
+        pos, tri, rast = ctx.saved_tensors
+        if not ctx.needs_input_grad[0] or (d_rast is None and d_db is None):
+            return None, None, None, None, None, None
+        B, H, W = rast.shape[0], rast.shape[1], rast.shape[2]
+        d_pos = torch.zeros_like(pos)
+        g = d_rast.to(torch.float32).contiguous() if d_rast is not None else None
+        if d_db is None:
+            L.check(L.lib().mcs_rasterize_bwd(*_pos_args(pos), tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W, g.data_ptr(), d_pos.data_ptr(),
+                                              L.stream_ptr()), "rasterize (backward)")
+        else:
+            h = d_db.to(torch.float32).contiguous()
+            L.check(L.lib().mcs_rasterize_bwd_db(*_pos_args(pos), tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W,
+                                                 g.data_ptr() if g is not None else None, h.data_ptr(), d_pos.data_ptr(), L.stream_ptr()),
+                    "rasterize_db (backward)")
+        return d_pos, None, None, None, None, None
+
+
 def _rasterize_args(name, mtx, pos, tri):
     """Validated (contiguous fp32 mtx, pos, tri) of a rasterize-style call; pos and tri are None together."""
     L.require_cuda(mtx)
@@ -79,15 +126,22 @@ def _rasterize_args(name, mtx, pos, tri):
     return m, pos.contiguous(), tri.contiguous()
 
 
-def rasterize(optix_ctx, mtx, resolution, pos=None, tri=None):
+def rasterize(optix_ctx, mtx, resolution, pos=None, tri=None, grad_db=False):
     """mtx: [B,4,4] clip-space transform (clip = mtx @ (p, 1), the `mtx_in` of render_mesh, render.py:289-293);
     resolution: (H, W).  Returns rast [B,H,W,4] fp32; a pixel whose ray hits nothing is all zeros.
 
     pos (clip-space vertices [V,4] or [B,V,4], fp32, equal to mtx @ (verts, 1) for the vertices the context's BVH was built from, e.g.
     `ru.xfm_points(v_pos[None], mtx)`) and tri (int32 [T,3]) make the result differentiable with respect to pos: the forward is the
     same ray-traced launch with a bit-identical output, and the backward maps d rast[...,0:2] to d pos through the perspective-correct
-    barycentrics of the clip-space triangle.  z/w and the id channel carry no gradient."""
+    barycentrics of the clip-space triangle.  z/w and the id channel carry no gradient.
+
+    grad_db=True returns (rast, rast_db): rast_db [B,H,W,4] = (du/dX, du/dY, dv/dX, dv/dY) in pixels at each pixel centre, for the
+    triangle in rast, from the clip-space triangle (so it needs pos and tri), differentiable with respect to pos."""
     m, pos, tri = _rasterize_args("rasterize", mtx, pos, tri)
+    if grad_db:
+        if pos is None:
+            raise ValueError("rasterize: grad_db=True needs pos and tri (the derivatives are those of the clip-space triangle)")
+        return _rasterize_db_func.apply(pos, tri, optix_ctx, m, resolution)
     if pos is None:
         return _rasterize_launch(optix_ctx, m, resolution)
     return _rasterize_func.apply(pos, tri, optix_ctx, m, resolution)
@@ -106,11 +160,16 @@ class DepthPeeler:
     so a ray through an edge shared by two triangles does not return the same surface twice.  Layer 0 equals `rasterize`; a pixel
     with no further surface is all zeros.  Every layer is an ordinary `rast`: given pos and tri it is differentiable with respect to
     pos exactly like `rasterize`, and `interpolate` and `antialias` take it.  The peeler keeps one fp32 per pixel, zeroed on entry.
-    Rebuilding or refitting the context's BVH between layers is an error, as it is for nvdiffrast's peeler to change the geometry."""
+    Rebuilding or refitting the context's BVH between layers is an error, as it is for nvdiffrast's peeler to change the geometry.
+    grad_db=True (needs pos and tri) makes every layer return (rast, rast_db) with that layer's screen-space derivatives, as
+    `rasterize(grad_db=True)`."""
 
-    def __init__(self, optix_ctx, mtx, resolution, pos=None, tri=None):
+    def __init__(self, optix_ctx, mtx, resolution, pos=None, tri=None, grad_db=False):
         self._m, self._pos, self._tri = _rasterize_args("DepthPeeler", mtx, pos, tri)
+        if grad_db and self._pos is None:
+            raise ValueError("DepthPeeler: grad_db=True needs pos and tri (the derivatives are those of the clip-space triangle)")
         self._ctx, self._res = optix_ctx, tuple(resolution)
+        self._grad_db = bool(grad_db)
         self._state = None
         self._version = None
 
@@ -125,11 +184,13 @@ class DepthPeeler:
         return False
 
     def rasterize_next_layer(self):
-        """Returns (rast [B,H,W,4], None), like dr.DepthPeeler.rasterize_next_layer without screen-space derivatives."""
+        """Returns (rast [B,H,W,4], rast_db [B,H,W,4]) with grad_db=True, else (rast, None), like dr.DepthPeeler.rasterize_next_layer."""
         if self._state is None:
             raise RuntimeError("DepthPeeler.rasterize_next_layer: only inside the peeler's `with` block")
         if self._ctx._version != self._version:
             raise RuntimeError("DepthPeeler.rasterize_next_layer: the BVH was rebuilt or refitted since the peeler started")
+        if self._grad_db:
+            return _rasterize_db_func.apply(self._pos, self._tri, self._ctx, self._m, self._res, self._state)
         if self._pos is None:
             return _rasterize_launch(self._ctx, self._m, self._res, self._state), None
         return _rasterize_func.apply(self._pos, self._tri, self._ctx, self._m, self._res, self._state), None
@@ -173,9 +234,80 @@ class _interpolate_func(torch.autograd.Function):
         return d_attr, None, None
 
 
-def interpolate(attr, rast, tri):
-    """attr [V,C] or [B,V,C], rast from `rasterize`, tri int32 [T,3].  Returns (out [B,H,W,C], None) like dr.interpolate."""
-    return _interpolate_func.apply(attr, rast, tri), None
+def _da_args(a, r, db, t, idx):
+    batched = a.dim() == 3
+    V, Cn = a.shape[-2], a.shape[-1]
+    n = Cn if idx is None else len(idx)
+    arr = None if idx is None else (ctypes.c_int32 * n)(*idx)       # passed by value into the kernel's parameters (no device tensor)
+    return (a.data_ptr(), V * Cn if batched else 0, V, Cn, t.data_ptr(), t.shape[0], r.data_ptr(), db.data_ptr(), r.shape[0], r.shape[1], r.shape[2],
+            n, arr), n
+
+
+class _interpolate_da_func(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, attr, rast_db, rast, tri, idx):
+        a = attr.to(torch.float32).contiguous(); db = rast_db.to(torch.float32).contiguous(); r = rast.to(torch.float32).contiguous()
+        t = tri.contiguous()
+        args, n = _da_args(a, r, db, t, idx)
+        out_da = torch.empty(r.shape[0], r.shape[1], r.shape[2], 2 * n, dtype=torch.float32, device=a.device)
+        L.check(L.lib().mcs_interpolate_da_fwd(*args, out_da.data_ptr(), L.stream_ptr()), "interpolate_da (forward)")
+        ctx.save_for_backward(a, db, r, t)
+        ctx.idx = idx
+        return out_da
+
+    @staticmethod
+    def backward(ctx, d_out_da):
+        a, db, r, t = ctx.saved_tensors
+        need_a, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (need_a or need_db):
+            return None, None, None, None, None
+        d_attr = torch.zeros_like(a) if need_a else None
+        d_db = torch.empty_like(db) if need_db else None
+        g = d_out_da.to(torch.float32).contiguous()
+        args, _ = _da_args(a, r, db, t, ctx.idx)
+        L.check(L.lib().mcs_interpolate_da_bwd(*args, g.data_ptr(), d_attr.data_ptr() if need_a else None, d_db.data_ptr() if need_db else None,
+                                               L.stream_ptr()), "interpolate_da (backward)")
+        return d_attr, d_db, None, None, None
+
+
+def _diff_attr_list(diff_attrs, C):
+    """None for 'all', else the validated tuple of attribute indices."""
+    if isinstance(diff_attrs, str):
+        if diff_attrs != "all":
+            raise ValueError("interpolate: diff_attrs must be 'all' or a list of attribute indices, got %r" % diff_attrs)
+        return None
+    idx = tuple(int(k) for k in diff_attrs)
+    if not idx or len(idx) > 32:
+        raise ValueError("interpolate: diff_attrs lists %d indices; 1 to 32 are allowed" % len(idx))
+    bad = [k for k in idx if not 0 <= k < C]
+    if bad:
+        raise ValueError("interpolate: diff_attrs index %d is outside [0, %d)" % (bad[0], C))
+    return idx
+
+
+def interpolate(attr, rast, tri, rast_db=None, diff_attrs=None):
+    """attr [V,C] or [B,V,C], rast from `rasterize`, tri int32 [T,3].  Returns (out [B,H,W,C], out_da) like dr.interpolate.
+
+    out_da is None unless diff_attrs is given: 'all', or a list of up to 32 attribute indices (order kept, repeats allowed).  It then
+    needs rast_db [B,H,W,4] (from `rasterize(grad_db=True)` or a `DepthPeeler(grad_db=True)` layer) and is [B,H,W,2n] in nvdiffrast's
+    layout: channels 2k and 2k+1 hold (dA/dX, dA/dY) of the k-th selected attribute A, zero where rast has no triangle.  out_da is
+    differentiable with respect to attr and rast_db (not rast: it does not depend on the barycentrics).  Semantics: csrc/raster.cu."""
+    if diff_attrs is None:
+        return _interpolate_func.apply(attr, rast, tri), None
+    if rast_db is None:
+        raise ValueError("interpolate: diff_attrs needs rast_db")
+    L.require_cuda(attr, rast, tri, rast_db)
+    if tri.dtype != torch.int32:
+        raise TypeError("interpolate: tri must be int32 [T,3]")
+    if rast.dim() != 4 or rast.shape[3] != 4:
+        raise ValueError("interpolate: rast must be [B,H,W,4], got %s" % (tuple(rast.shape),))
+    if tuple(rast_db.shape) != tuple(rast.shape):
+        raise ValueError("interpolate: rast_db must be [B,H,W,4] like rast %s, got %s" % (tuple(rast.shape), tuple(rast_db.shape)))
+    if attr.dim() not in (2, 3):
+        raise ValueError("interpolate: attr must be [V,C] or [B,V,C], got %s" % (tuple(attr.shape),))
+    idx = _diff_attr_list(diff_attrs, attr.shape[-1])
+    out = _interpolate_func.apply(attr, rast, tri)
+    return out, _interpolate_da_func.apply(attr, rast_db, rast.detach(), tri, idx)
 
 
 def antialias_topology(tri):

@@ -302,6 +302,30 @@ int mcs_hashgrid_fwd(const float *x, int64_t n, const float *params, const mcs_h
 int mcs_hashgrid_bwd(const float *x, int64_t n, const float *params, const mcs_hashgrid_levels *lv, const float *d_out, float *d_params,
                      float *d_x, mcs_stream stream);
 
+/* ---- filtered, mip-mapped texture sampling: stands in for nvdiffrast's `dr.texture` in Texture2D.sample and its mip chain's backward
+ *      (render/texture.py:27-30,57-68), the regulariser taps (render/render.py:54,75-95) and the probe look-ups (render/light.py:64,76);
+ *      semantics in csrc/texture.cu.  The level table is passed by value: level k is ptr[k], [Bt, h[k], w[k], C] fp32 contiguous, with
+ *      h[k] = max(1, h[0] >> k), w[k] = max(1, w[0] >> k); batch_stride[k] = 0 shares the level over the minibatch, else h*w*C (every
+ *      level alike).  uv [B,H,W,2], uv_da [B,H,W,4] (du/dX, du/dY, dv/dX, dv/dY; required by linear-mipmap-linear, else ignored), out and
+ *      d_out [B,H,W,C], contiguous fp32; uv 8-byte and uv_da 16-byte aligned.  MCS_TEX_LINEAR reads level 0 only.
+ *      The backward adds into d_tex[k] (a HOST array of n_levels device pointers, caller-zeroed, float atomics; the array or any entry may be
+ *      null) and overwrites d_uv [B,H,W,2] and d_uv_da [B,H,W,4] (deterministic; each may be null; d_uv_da is only written with
+ *      MCS_TEX_LINEAR_MIPMAP_LINEAR; at least one gradient).  One launch per call, no host sync, no allocation. */
+enum { MCS_TEX_LINEAR = 0, MCS_TEX_LINEAR_MIPMAP_LINEAR = 1 };
+enum { MCS_TEX_WRAP = 0, MCS_TEX_CLAMP = 1 };
+typedef struct mcs_texture_levels {
+    int32_t n_levels;          /* 1..16 */
+    int32_t C;                 /* channels, >= 1 */
+    const float *ptr[16];
+    int32_t h[16];
+    int32_t w[16];
+    int64_t batch_stride[16];  /* elements */
+} mcs_texture_levels;
+int mcs_texture_fwd(const mcs_texture_levels *tex, const float *uv, const float *uv_da, int32_t B, int32_t H, int32_t W, int32_t filter_mode,
+                    int32_t boundary_mode, float *out, mcs_stream stream);
+int mcs_texture_bwd(const mcs_texture_levels *tex, const float *uv, const float *uv_da, int32_t B, int32_t H, int32_t W, int32_t filter_mode,
+                    int32_t boundary_mode, const float *d_out, float *const *d_tex, float *d_uv, float *d_uv_da, mcs_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -14,7 +14,7 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_PKG, "csrc")
 _LIBDIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
-SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu"]
+SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
@@ -63,6 +63,11 @@ def build(force=False, verbose=False):
 
 class mcs_hashgrid_levels(C.Structure):
     _fields_ = [("n_levels", C.c_int32), ("offset", C.c_uint32 * 17), ("res", C.c_uint32 * 16), ("scale", C.c_float * 16), ("dense_mask", C.c_uint32)]
+
+
+class mcs_texture_levels(C.Structure):
+    _fields_ = [("n_levels", C.c_int32), ("C", C.c_int32), ("ptr", C.c_void_p * 16), ("h", C.c_int32 * 16), ("w", C.c_int32 * 16),
+                ("batch_stride", C.c_int64 * 16)]
 
 
 class mcs_tensor(C.Structure):
@@ -137,6 +142,8 @@ _SIGS = {
     "mcs_antialias_bwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
     "mcs_hashgrid_fwd": ([_P, C.c_int64, _P, _P, _P, _P], C.c_int),
     "mcs_hashgrid_bwd": ([_P, C.c_int64, _P, _P, _P, _P, _P, _P], C.c_int),
+    "mcs_texture_fwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P, _P], C.c_int),
+    "mcs_texture_bwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P] * 5, C.c_int),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 
@@ -166,7 +173,8 @@ def lib():
 # and for meshes of 5 to 16 384 triangles the shadow view's clustering and emission.
 LAUNCHES = collections.Counter()
 _KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "rasterize_peel": 2,
-                     "antialias_topology": 2, "hashgrid_bwd_both": 2}
+                     "antialias_topology": 2, "hashgrid_bwd_both": 2,
+                     "texture_fwd": 1, "texture_bwd": 1}
 
 
 def check(status, what):

@@ -11,7 +11,10 @@ antialiasing of Laine et al. 2020, the only path from coverage (alpha) to vertex
 back-to-front `composite_buffer` needs.  Screen-space derivatives come in nvdiffrast's layout: `rasterize(grad_db=True)` and
 `DepthPeeler(grad_db=True)` also return `rast_db` (du/dX, du/dY, dv/dX, dv/dY in pixels, from the clip-space triangle), and
 `interpolate(..., rast_db=, diff_attrs=)` returns the attribute derivatives `out_da` that render_layer turns into the denoiser's depth
-guide (render.py:225-234)."""
+guide (render.py:225-234).  `texture` is nvdiffrast's filtered look-up with its signature, in the modes the reference calls: bilinear
+('linear') and trilinear on a mip chain with the level of detail taken from `uv_da` ('linear-mipmap-linear', e.g. `gb_texc_deriv`),
+'wrap' or 'clamp' borders, differentiable with respect to the texture, every mip level, uv and uv_da (Texture2D.sample, texture.py:57-68,
+its mip chain's backward and the regulariser taps of render.py)."""
 import ctypes
 
 import torch
@@ -375,6 +378,122 @@ def antialias(color, rast, pos, tri, topology=None):
             raise ValueError("antialias: topology has %d rows for %d triangles" % (topology.shape[0], tri.shape[0]))
     return _antialias_func.apply(color.to(torch.float32).contiguous(), pos.contiguous(), rast.detach().contiguous(), tri.contiguous(),
                                  topology.contiguous())
+
+
+_TEX_FILTERS = {"linear": 0, "linear-mipmap-linear": 1}
+_TEX_BOUNDARIES = {"wrap": 0, "clamp": 1}
+_TEX_MAX_LEVELS = 16
+
+
+def _tex_levels(levels):
+    lv = L.mcs_texture_levels()
+    lv.n_levels, lv.C = len(levels), levels[0].shape[3]
+    for k, t in enumerate(levels):
+        lv.ptr[k], lv.h[k], lv.w[k] = t.data_ptr(), t.shape[1], t.shape[2]
+        lv.batch_stride[k] = 0 if t.shape[0] == 1 else t.shape[1] * t.shape[2] * t.shape[3]
+    return lv
+
+
+class _texture_func(torch.autograd.Function):
+    """inputs: filter and boundary codes, uv, uv_da (None in 'linear'), then the levels (level 0 first); one launch each way."""
+    @staticmethod
+    def forward(ctx, filt, bnd, uv, uv_da, *levels):
+        B, H, W = uv.shape[0], uv.shape[1], uv.shape[2]
+        out = torch.empty(B, H, W, levels[0].shape[3], dtype=torch.float32, device=uv.device)
+        L.check(L.lib().mcs_texture_fwd(ctypes.byref(_tex_levels(levels)), uv.data_ptr(), uv_da.data_ptr() if uv_da is not None else None, B, H, W,
+                                        filt, bnd, out.data_ptr(), L.stream_ptr()), "texture_fwd")
+        ctx.save_for_backward(uv, uv_da, *levels)
+        ctx.codes = (filt, bnd)
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        uv, uv_da, *levels = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        if not any(need[2:]):
+            return (None,) * len(need)
+        filt, bnd = ctx.codes
+        d_uv = torch.empty_like(uv) if need[2] else None
+        d_uv_da = torch.empty_like(uv_da) if need[3] else None
+        d_levels = [torch.zeros_like(t) if need[4 + k] else None for k, t in enumerate(levels)]
+        ptrs = (ctypes.c_void_p * len(levels))(*[t.data_ptr() if t is not None else None for t in d_levels])
+        g = dout.to(torch.float32).contiguous()
+        B, H, W = uv.shape[0], uv.shape[1], uv.shape[2]
+        L.check(L.lib().mcs_texture_bwd(ctypes.byref(_tex_levels(levels)), uv.data_ptr(), uv_da.data_ptr() if uv_da is not None else None, B, H, W,
+                                        filt, bnd, g.data_ptr(), ptrs, d_uv.data_ptr() if d_uv is not None else None,
+                                        d_uv_da.data_ptr() if d_uv_da is not None else None, L.stream_ptr()), "texture_bwd")
+        return (None, None, d_uv, d_uv_da, *d_levels)
+
+
+def _check_tex(t, what, Bt=None, C=None):
+    if not isinstance(t, torch.Tensor) or t.dim() != 4:
+        raise ValueError("texture: %s must be a [Bt,H,W,C] tensor, got %s" % (what, tuple(t.shape) if isinstance(t, torch.Tensor) else type(t)))
+    if t.dtype != torch.float32:
+        raise ValueError("texture: %s must be fp32, got %s" % (what, t.dtype))
+    if t.shape[1] < 1 or t.shape[2] < 1 or t.shape[3] < 1:
+        raise ValueError("texture: %s has an empty dimension %s" % (what, tuple(t.shape)))
+    if Bt is not None and (t.shape[0] != Bt or t.shape[3] != C):
+        raise ValueError("texture: %s is %s; its minibatch and channels must be those of tex (%d, %d)" % (what, tuple(t.shape), Bt, C))
+
+
+def texture(tex, uv, uv_da=None, mip_level_bias=None, mip=None, filter_mode='auto', boundary_mode='wrap', max_mip_level=None):
+    """Filtered texture look-up with nvdiffrast's signature, the stand-in for `dr.texture` in the modes the reference calls.
+
+    tex [Bt,H,W,C] fp32 (any C >= 1; Bt = 1 is shared by the whole minibatch, else Bt = B), uv [B,h,w,2], uv_da [B,h,w,4] =
+    (du/dX, du/dY, dv/dX, dv/dY) as `interpolate(..., diff_attrs='all')` returns them for a 2-channel texture coordinate.  Returns
+    [B,h,w,C] fp32.  filter_mode 'linear' (level 0 only) or 'linear-mipmap-linear' (trilinear on the chain tex, mip[0], mip[1], ...,
+    level k of max(1, H >> k) x max(1, W >> k), up to 16 levels; the chain may stop early); 'auto' is the latter when uv_da is given.
+    mip=None in a mipmap mode is accepted for a 1x1 tex only (a one-level chain); build the chain of a larger texture and pass it.
+    boundary_mode 'wrap' or 'clamp'.  Differentiable with respect to tex, every mip level, uv and uv_da ('linear' ignores mip and uv_da).
+    Not provided (ValueError): 'nearest', 'linear-mipmap-nearest', 'zero', 'cube', mip_level_bias, max_mip_level.  Semantics,
+    including the level of detail: csrc/texture.cu."""
+    if filter_mode == 'auto':
+        filter_mode = 'linear-mipmap-linear' if uv_da is not None else 'linear'
+    if filter_mode not in _TEX_FILTERS:
+        raise ValueError("texture: filter_mode %r is not provided (only 'linear' and 'linear-mipmap-linear')" % (filter_mode,))
+    if boundary_mode not in _TEX_BOUNDARIES:
+        raise ValueError("texture: boundary_mode %r is not provided (only 'wrap' and 'clamp')" % (boundary_mode,))
+    if mip_level_bias is not None or max_mip_level is not None:
+        raise ValueError("texture: mip_level_bias and max_mip_level are not provided")
+    mipmap = filter_mode == 'linear-mipmap-linear'
+    _check_tex(tex, "tex")
+    Bt, H0, W0, C = tex.shape
+    if not isinstance(uv, torch.Tensor) or uv.dim() != 4 or uv.shape[3] != 2:
+        raise ValueError("texture: uv must be [B,h,w,2], got %s" % (tuple(uv.shape) if isinstance(uv, torch.Tensor) else type(uv),))
+    if uv.dtype != torch.float32:
+        raise ValueError("texture: uv must be fp32, got %s" % uv.dtype)
+    B = uv.shape[0]
+    if Bt not in (1, B):
+        raise ValueError("texture: tex minibatch %d must be 1 or that of uv (%d)" % (Bt, B))
+    levels = [tex]
+    if mipmap:
+        if uv_da is None:
+            raise ValueError("texture: filter_mode 'linear-mipmap-linear' needs uv_da")
+        if not isinstance(uv_da, torch.Tensor) or tuple(uv_da.shape) != tuple(uv.shape[:3]) + (4,):
+            raise ValueError("texture: uv_da must be [B,h,w,4] like uv %s, got %s" % (tuple(uv.shape), tuple(uv_da.shape) if isinstance(uv_da, torch.Tensor) else type(uv_da)))
+        if uv_da.dtype != torch.float32:
+            raise ValueError("texture: uv_da must be fp32, got %s" % uv_da.dtype)
+        if mip is None:
+            if (H0, W0) != (1, 1):
+                raise ValueError("texture: filter_mode 'linear-mipmap-linear' on a %d x %d texture needs its chain: pass mip=[level 1, ...]" % (H0, W0))
+        else:
+            mip = list(mip)
+            if len(mip) + 1 > _TEX_MAX_LEVELS:
+                raise ValueError("texture: %d levels; at most %d are supported" % (len(mip) + 1, _TEX_MAX_LEVELS))
+            for k, m in enumerate(mip, 1):
+                _check_tex(m, "mip[%d]" % (k - 1), Bt, C)
+                want = (max(1, H0 >> k), max(1, W0 >> k))
+                if tuple(m.shape[1:3]) != want:
+                    raise ValueError("texture: mip[%d] (level %d) is %d x %d, expected %d x %d" % (k - 1, k, m.shape[1], m.shape[2], *want))
+            levels += mip
+    else:
+        uv_da = None
+    L.require_cuda(uv, *levels)
+    if uv_da is not None:
+        L.require_cuda(uv_da)
+        uv_da = uv_da.contiguous()
+    return _texture_func.apply(_TEX_FILTERS[filter_mode], _TEX_BOUNDARIES[boundary_mode], uv.contiguous(), uv_da,
+                               *[t.contiguous() for t in levels])
 
 
 class _texel_fetch_func(torch.autograd.Function):

@@ -9,7 +9,7 @@ name=$1; shift
 out="$root/nvdiffrecmc_b200/lib/variants"
 mkdir -p "$out/obj_$name"
 cd "$src"
-for f in core elementwise denoise bvh envshade lossmesh light raster hashgrid; do
+for f in core elementwise denoise bvh envshade lossmesh light raster hashgrid texture; do
   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Xcompiler -fPIC "$@" -c $f.cu -o "$out/obj_$name/$f.o" &
 done
 wait

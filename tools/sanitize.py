@@ -68,6 +68,13 @@ enc = Encoding(3, {"otype": "HashGrid", "n_levels": 5, "log2_hashmap_size": 9, "
 xh = (torch.rand(1000, 3, device=dev) * 2 - 0.5).requires_grad_(True)
 enc(xh).sum().backward()
 enc(xh.detach()).sum().backward()
+# filtered texture look-up: 'linear' / 'clamp' on a per-batch 3-channel texture, 'linear-mipmap-linear' / 'wrap' on a custom 4-channel chain
+from nvdiffrecmc_b200.raster import texture
+uvt = (torch.rand(2, 9, 11, 2, device=dev) * 1.6 - 0.3).requires_grad_(True)
+dat = (torch.randn(2, 9, 11, 4, device=dev) * 0.2).requires_grad_(True)
+texture(torch.rand(2, 5, 7, 3, device=dev, requires_grad=True), uvt, filter_mode="linear", boundary_mode="clamp").sum().backward()
+mipc = [torch.rand(1, max(1, 12 >> k), max(1, 20 >> k), 4, device=dev, requires_grad=True) for k in range(5)]
+texture(mipc[0], uvt, dat, mip=mipc[1:]).sum().backward()
 if os.environ.get("MCS_EW_TMA"):
     B, H, W = 1, 400, 400          # 160 000 px = 312 tiles of 512 px (>= 2 x 132) + a ragged tail
     ins = [torch.rand(B, H, W, 3, device=dev).requires_grad_(True) for _ in range(6)]

@@ -47,6 +47,33 @@ __host__ __device__ __forceinline__ f3 cross(f3 a, f3 b) { return F3(a.y * b.z -
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fminf(hi, fmaxf(lo, x)); }
 
 // ---------------------------------------------------------------------------------------------
+// Warp-grouped atomics: lanes of a warp whose values go to the same addresses sum them first, and
+// one lane issues the atomics for the group.  The group is peers = __match_any_sync(0xFFFFFFFF, key):
+// every lane of the warp must reach that match (no early exit before it), and a lane with nothing
+// to scatter passes a key no live lane can have, so that it groups with no one and then leaves.
+// The live lanes of a group call warp_group_sum together: it sums v over the group in lane order
+// (shuffles) and returns true in the lane that issues the atomics, the lowest of the group.  A lane
+// alone in its group keeps its values and returns true.
+// ---------------------------------------------------------------------------------------------
+template <int N>
+__device__ __forceinline__ bool warp_group_sum(unsigned peers, float (&v)[N])
+{
+    const unsigned lane = threadIdx.x & 31u;
+    if (peers == (1u << lane)) return true;
+    float s[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) s[k] = 0.0f;
+    for (unsigned m = peers; m; m &= m - 1) {
+        const int src = __ffs(m) - 1;
+#pragma unroll
+        for (int k = 0; k < N; ++k) s[k] += __shfl_sync(peers, v[k], src);
+    }
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] = s[k];
+    return (int)lane == __ffs(peers) - 1;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Strided NHWC accessor built from mcs_tensor (size-1 dims broadcast => stride 0)
 // ---------------------------------------------------------------------------------------------
 struct TView {

@@ -68,26 +68,14 @@ __device__ __forceinline__ void hg_weights(const Cell &cl, int c, float w1[3])
 }
 
 // d params of one corner, one vector atomic (red.global.add.v2.f32) for both features.  With `agg`, lanes of the warp that scatter into
-// the same entry sum their pairs with shuffles (lane order) and one lane issues the atomic; every lane of the warp must then call this
-// (live = false for a lane without a gradient).
+// the same entry are grouped (warp_group_sum); every lane of the warp must then call this (live = false for a lane without a gradient).
 __device__ __forceinline__ void hg_scatter(float2 *base, uint32_t idx, float2 g, bool live, bool agg)
 {
     if (agg) {
-        const unsigned lane = threadIdx.x & 31u;
-        const uint64_t key = live ? (uint64_t)idx : (1ull << 32) + lane;
-        const unsigned peers = __match_any_sync(0xFFFFFFFFu, key);
+        const unsigned peers = __match_any_sync(0xFFFFFFFFu, live ? (uint64_t)idx : (1ull << 32) + (threadIdx.x & 31u));
         if (!live) return;
-        if (peers != (1u << lane)) {
-            float sx = 0.0f, sy = 0.0f;
-            for (unsigned m = peers; m; m &= m - 1) {
-                const int src = __ffs(m) - 1;
-                sx = __fadd_rn(sx, __shfl_sync(peers, g.x, src));
-                sy = __fadd_rn(sy, __shfl_sync(peers, g.y, src));
-            }
-            if ((int)lane != __ffs(peers) - 1) return;
-            g = make_float2(sx, sy);
-        }
-        atomicAdd(base + idx, g);
+        float v[2] = {g.x, g.y};
+        if (warp_group_sum(peers, v)) atomicAdd(base + idx, make_float2(v[0], v[1]));
     } else if (live) {
         atomicAdd(base + idx, g);
     }

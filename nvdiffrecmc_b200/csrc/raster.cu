@@ -40,7 +40,7 @@
 //                       ds_i/dpx = y_{i+1} w_{i+2} - w_{i+1} y_{i+2},   ds_i/dpy = w_{i+1} x_{i+2} - x_{i+1} w_{i+2},
 //                       du/dpx = (ds0/dpx - u dS/dpx) / S  (likewise py, and v with s1),   d/dX = (2/W) d/dpx,  d/dY = (2/H) d/dpy.
 //                     All four channels are 0 for background, ids >= T and S == 0.  Every operation is explicitly rounded in one fixed
-//                     order (the fp32 build of oracle/raster_db.c evaluates the same order), so rast_db is bit-reproducible.  A vertex
+//                     order (the fp32 build of oracle/geometry.c evaluates the same order), so rast_db is bit-reproducible.  A vertex
 //                     with w <= 0 needs no special case: the projective formula holds wherever the pixel has a hit.  One launch after
 //                     rasterize or any peel layer; k_rasterize is unchanged.
 //   k_interpolate_da: out_da[b,y,x,2k:2k+2] = (dA/dX, dA/dY) of the k-th selected attribute A (attribute-major, nvdiffrast's layout):
@@ -93,12 +93,19 @@ __device__ __forceinline__ void mul4(const float *__restrict__ m, float x, float
     for (int r = 0; r < 4; ++r) o[r] = fmaf(__ldg(m + 4 * r), x, fmaf(__ldg(m + 4 * r + 1), y, fmaf(__ldg(m + 4 * r + 2), z, __ldg(m + 4 * r + 3) * w)));
 }
 
+// image b, row iy and column ix of flat pixel index i of a [B,H,W] image
+__device__ __forceinline__ void px_decode(int64_t i, int H, int W, int &b, int &iy, int &ix)
+{
+    ix = (int)(i % W); const int64_t t = i / W; iy = (int)(t % H); b = (int)(t / H);
+}
+
 __global__ void __launch_bounds__(128) k_rasterize(const RasterParams p)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t n = (int64_t)p.B * p.H * p.W;
     if (i >= n) return;
-    const int ix = (int)(i % p.W); const int64_t t_ = i / p.W; const int iy = (int)(t_ % p.H), b = (int)(t_ / p.H);
+    int b, iy, ix;
+    px_decode(i, p.H, p.W, b, iy, ix);
     const float x = ((float)ix + 0.5f) / (float)p.W * 2.0f - 1.0f, y = ((float)iy + 0.5f) / (float)p.H * 2.0f - 1.0f;
     float a[4], c[4];
     mul4(p.inv + 16 * b, x, y, -1.0f, 1.0f, a);
@@ -213,16 +220,13 @@ struct InterpDaParams {
 
 // out_da and its backward (semantics in the file header).  Differences and products are explicitly rounded so the forward and
 // d rast_db equal the fp32 oracle bit for bit.
-// d attr: with MCS_DA_AGG, lanes of a warp that hit the same triangle of the same image sum their per-vertex terms with shuffles
-// (__match_any_sync groups, as k_rasterize_bwd) and one lane issues the atomics.
-#ifndef MCS_DA_AGG
-#define MCS_DA_AGG 1
-#endif
+// d attr: lanes of a warp that hit the same triangle of the same image are grouped once per pixel (as k_rasterize_bwd) and sum their
+// per-vertex terms once per selected attribute (warp_group_sum).
 template <bool BWD>
 __global__ void __launch_bounds__(256) k_interpolate_da(const InterpDaParams p)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const bool agg = BWD && MCS_DA_AGG && p.dattr;      // then every lane of the warp reaches __match_any_sync (no early exit before it)
+    const bool agg = BWD && p.dattr;      // then every lane of the warp reaches __match_any_sync (no early exit before it)
     if (i >= p.npx && !agg) return;
     int id = -1;
     if (i < p.npx) {
@@ -261,20 +265,11 @@ __global__ void __launch_bounds__(256) k_interpolate_da(const InterpDaParams p)
         } else {
             const float gX = __ldg(p.dout_da + (i * n + k) * 2), gY = __ldg(p.dout_da + (i * n + k) * 2 + 1);
             if (p.dattr) {
-                float a0 = gX * db.x + gY * db.y, a1 = gX * db.z + gY * db.w;
-                bool issue = gX != 0.0f || gY != 0.0f;
-                if (agg && peers != (1u << lane)) {
-                    float s0 = 0.0f, s1 = 0.0f;
-                    for (unsigned m = peers; m; m &= m - 1) {
-                        const int src = __ffs(m) - 1;
-                        s0 += __shfl_sync(peers, a0, src); s1 += __shfl_sync(peers, a1, src);
-                    }
-                    a0 = s0; a1 = s1;
-                    issue = (int)lane == __ffs(peers) - 1 && (a0 != 0.0f || a1 != 0.0f);
-                }
+                float a[2] = {gX * db.x + gY * db.y, gX * db.z + gY * db.w};
+                const bool issue = peers == (1u << lane) ? gX != 0.0f || gY != 0.0f : warp_group_sum(peers, a) && (a[0] != 0.0f || a[1] != 0.0f);
                 if (issue) {
                     float *D = p.dattr + base;
-                    atomicAdd(D + (size_t)i0 * p.C + c, a0); atomicAdd(D + (size_t)i1 * p.C + c, a1); atomicAdd(D + (size_t)i2 * p.C + c, -(a0 + a1));
+                    atomicAdd(D + (size_t)i0 * p.C + c, a[0]); atomicAdd(D + (size_t)i1 * p.C + c, a[1]); atomicAdd(D + (size_t)i2 * p.C + c, -(a[0] + a[1]));
                 }
             }
             if (p.ddb) {
@@ -302,7 +297,36 @@ struct RastBwdParams {
 // NDC coordinate of pixel centre i of n (image row iy -> NDC y = (iy + 0.5) / H * 2 - 1, as k_rasterize), explicitly rounded
 __device__ __forceinline__ float px_ndc(int i, int n) { return __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn((float)i, 0.5f), (float)n), 2.0f), 1.0f); }
 
-// rast_db (file header): one thread per pixel, explicitly rounded in the order of oracle/raster_db.c's orc_rast_db
+// a = (x - px w, y - py w) of clip-space vertex (x, y, w) seen from NDC point (px, py), explicitly rounded
+__device__ __forceinline__ float2 clip_a(float x, float y, float w, float px, float py)
+{
+    return make_float2(__fsub_rn(x, __fmul_rn(px, w)), __fsub_rn(y, __fmul_rn(py, w)));
+}
+
+// edge function a_A x a_B, explicitly rounded
+__device__ __forceinline__ float clip_edge(float2 a, float2 b) { return __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)); }
+
+// triangle id of the clip-space mesh seen from pixel centre (px, py) (file header): vertex ids, (x, y, w), a_k, s_k = a_{k+1} x a_{k+2}
+// and S = (s0 + s1) + s2
+struct ClipTri { int vi[3]; float x[3], y[3], w[3]; float2 a[3]; float s[3], S; };
+
+__device__ __forceinline__ ClipTri clip_tri(const float *P, const int32_t *tris, int id, float px, float py)
+{
+    ClipTri c;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        c.vi[k] = __ldg(tris + 3 * (size_t)id + k);
+        const float *q = P + 4 * (size_t)c.vi[k];
+        c.x[k] = __ldg(q); c.y[k] = __ldg(q + 1); c.w[k] = __ldg(q + 3);
+        c.a[k] = clip_a(c.x[k], c.y[k], c.w[k], px, py);
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) c.s[k] = clip_edge(c.a[k == 2 ? 0 : k + 1], c.a[k == 0 ? 2 : k - 1]);
+    c.S = __fadd_rn(__fadd_rn(c.s[0], c.s[1]), c.s[2]);
+    return c;
+}
+
+// rast_db (file header): one thread per pixel, explicitly rounded in the order of oracle/geometry.c's orc_rast_db
 __global__ void __launch_bounds__(256) k_rast_db(const RastBwdParams p)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -312,30 +336,20 @@ __global__ void __launch_bounds__(256) k_rast_db(const RastBwdParams p)
     const int id = (int)r.w - 1;
     float4 out = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     if (id >= 0 && id < p.T) {
-        const int ix = (int)(i % p.W); const int64_t t_ = i / p.W; const int iy = (int)(t_ % p.H), b = (int)(t_ / p.H);
-        const float px = px_ndc(ix, p.W), py = px_ndc(iy, p.H);
-        const float *P = p.pos + (int64_t)b * p.pos_bs;
-        float x[3], y[3], w[3], ax[3], ay[3];
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            const float *q = P + 4 * (size_t)__ldg(p.tris + 3 * (size_t)id + k);
-            x[k] = __ldg(q); y[k] = __ldg(q + 1); w[k] = __ldg(q + 3);
-            ax[k] = __fsub_rn(x[k], __fmul_rn(px, w[k])); ay[k] = __fsub_rn(y[k], __fmul_rn(py, w[k]));
-        }
-        const float s0 = __fsub_rn(__fmul_rn(ax[1], ay[2]), __fmul_rn(ay[1], ax[2]));
-        const float s1 = __fsub_rn(__fmul_rn(ax[2], ay[0]), __fmul_rn(ay[2], ax[0]));
-        const float s2 = __fsub_rn(__fmul_rn(ax[0], ay[1]), __fmul_rn(ay[0], ax[1]));
-        const float S = __fadd_rn(__fadd_rn(s0, s1), s2);
+        int b, iy, ix;
+        px_decode(i, p.H, p.W, b, iy, ix);
+        const ClipTri c = clip_tri(p.pos + (int64_t)b * p.pos_bs, p.tris, id, px_ndc(ix, p.W), px_ndc(iy, p.H));
+        const float S = c.S;
         if (S != 0.0f) {
             float dx[3], dy[3];
 #pragma unroll
             for (int k = 0; k < 3; ++k) {
                 const int k1 = k == 2 ? 0 : k + 1, k2 = k == 0 ? 2 : k - 1;
-                dx[k] = __fsub_rn(__fmul_rn(y[k1], w[k2]), __fmul_rn(w[k1], y[k2]));
-                dy[k] = __fsub_rn(__fmul_rn(w[k1], x[k2]), __fmul_rn(x[k1], w[k2]));
+                dx[k] = __fsub_rn(__fmul_rn(c.y[k1], c.w[k2]), __fmul_rn(c.w[k1], c.y[k2]));
+                dy[k] = __fsub_rn(__fmul_rn(c.w[k1], c.x[k2]), __fmul_rn(c.x[k1], c.w[k2]));
             }
             const float dSx = __fadd_rn(__fadd_rn(dx[0], dx[1]), dx[2]), dSy = __fadd_rn(__fadd_rn(dy[0], dy[1]), dy[2]);
-            const float u = __fdiv_rn(s0, S), v = __fdiv_rn(s1, S);
+            const float u = __fdiv_rn(c.s[0], S), v = __fdiv_rn(c.s[1], S);
             const float sx = __fdiv_rn(2.0f, (float)p.W), sy = __fdiv_rn(2.0f, (float)p.H);
             out.x = __fmul_rn(__fdiv_rn(__fsub_rn(dx[0], __fmul_rn(u, dSx)), S), sx);
             out.y = __fmul_rn(__fdiv_rn(__fsub_rn(dy[0], __fmul_rn(u, dSy)), S), sy);
@@ -346,9 +360,9 @@ __global__ void __launch_bounds__(256) k_rast_db(const RastBwdParams p)
     p.rast_db[i] = out;
 }
 
-// Lanes of a warp that hit the same triangle of the same image sum their 9 vertex gradients with shuffles (__match_any_sync groups,
-// summed in lane order) and one lane issues the atomics: 0.093 ms against 0.354 ms with 9 atomics per pixel at 8 x 512^2 on the bench
-// mesh (H100 80GB HBM3, 400 W), where consecutive pixels of a row mostly share a triangle.
+// Lanes of a warp that hit the same triangle of the same image sum their 9 vertex gradients with shuffles (warp_group_sum) and one
+// lane issues the atomics: 0.093 ms against 0.354 ms with 9 atomics per pixel at 8 x 512^2 on the bench mesh (H100 80GB HBM3, 400 W),
+// where consecutive pixels of a row mostly share a triangle.
 // DB: d rast (may be null) and d rast_db; without DB this is the d rast-only kernel.
 template <bool DB>
 __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
@@ -356,7 +370,7 @@ __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t n = (int64_t)p.B * p.H * p.W;
     int id = -1, b = 0;
-    float gx[3] = {0.0f, 0.0f, 0.0f}, gy[3] = {0.0f, 0.0f, 0.0f}, gw[3] = {0.0f, 0.0f, 0.0f};
+    float gv[3][3] = {};         // (d x, d y, d w) of vertex k
     int vi[3] = {0, 0, 0};
     if (i < n) {
         const float4 r = __ldg(p.rast + i);
@@ -370,36 +384,28 @@ __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
         }
         if (id >= p.T || zero) id = -1;
         if (id >= 0) {
-            const int ix = (int)(i % p.W); const int64_t t_ = i / p.W; const int iy = (int)(t_ % p.H); b = (int)(t_ / p.H);
+            int iy, ix;
+            px_decode(i, p.H, p.W, b, iy, ix);
             const float px = px_ndc(ix, p.W), py = px_ndc(iy, p.H);
-            const float *P = p.pos + (int64_t)b * p.pos_bs;
-            float ax[3], ay[3], x[3], y[3], wv[3];
+            const ClipTri c = clip_tri(p.pos + (int64_t)b * p.pos_bs, p.tris, id, px, py);
 #pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                vi[k] = __ldg(p.tris + 3 * (size_t)id + k);
-                const float *q = P + 4 * (size_t)vi[k];
-                const float w = __ldg(q + 3);
-                ax[k] = __fsub_rn(__ldg(q), __fmul_rn(px, w)); ay[k] = __fsub_rn(__ldg(q + 1), __fmul_rn(py, w));
-                if (DB) { x[k] = __ldg(q); y[k] = __ldg(q + 1); wv[k] = w; }
-            }
-            const float s0 = __fsub_rn(__fmul_rn(ax[1], ay[2]), __fmul_rn(ay[1], ax[2]));
-            const float s1 = __fsub_rn(__fmul_rn(ax[2], ay[0]), __fmul_rn(ay[2], ax[0]));
-            const float s2 = __fsub_rn(__fmul_rn(ax[0], ay[1]), __fmul_rn(ay[0], ax[1]));
-            const float S = __fadd_rn(__fadd_rn(s0, s1), s2);
+            for (int k = 0; k < 3; ++k) vi[k] = c.vi[k];
+            const float S = c.S;
             if (S == 0.0f) {
                 id = -1;
             } else {
-                const float u = s0 / S, v = s1 / S, G = g.x * u + g.y * v;
+                const float u = c.s[0] / S, v = c.s[1] / S, G = g.x * u + g.y * v;
                 float gs[3] = {(g.x - G) / S, (g.y - G) / S, -G / S};
                 float ex[3], ey[3];
                 if (DB) {
-                    // L = sum_{c = u, v; p = px, py} h_cp (ds_c/dp - c dS/dp) / S with h the pixel-scaled d rast_db
+                    // L = sum_{c = u, v; p = px, py} h_cp (ds_c/dp - c dS/dp) / S with h the pixel-scaled d rast_db; the ds_i/dp terms
+                    // are contractible here, unlike k_rast_db's
                     float dx[3], dy[3];
 #pragma unroll
                     for (int k = 0; k < 3; ++k) {
                         const int k1 = k == 2 ? 0 : k + 1, k2 = k == 0 ? 2 : k - 1;
-                        dx[k] = y[k1] * wv[k2] - wv[k1] * y[k2];
-                        dy[k] = wv[k1] * x[k2] - x[k1] * wv[k2];
+                        dx[k] = c.y[k1] * c.w[k2] - c.w[k1] * c.y[k2];
+                        dy[k] = c.w[k1] * c.x[k2] - c.x[k1] * c.w[k2];
                     }
                     const float dSx = dx[0] + dx[1] + dx[2], dSy = dy[0] + dy[1] + dy[2];
                     const float sx = 2.0f / (float)p.W, sy = 2.0f / (float)p.H;
@@ -415,40 +421,31 @@ __global__ void __launch_bounds__(256) k_rasterize_bwd(const RastBwdParams p)
 #pragma unroll
                 for (int k = 0; k < 3; ++k) {
                     const int k1 = k == 2 ? 0 : k + 1, k2 = k == 0 ? 2 : k - 1;
-                    gx[k] = gs[k2] * ay[k1] - gs[k1] * ay[k2];
-                    gy[k] = gs[k1] * ax[k2] - gs[k2] * ax[k1];
-                    gw[k] = -px * gx[k] - py * gy[k];
+                    float gx = gs[k2] * c.a[k1].y - gs[k1] * c.a[k2].y;
+                    float gy = gs[k1] * c.a[k2].x - gs[k2] * c.a[k1].x;
+                    float gw = -px * gx - py * gy;
                     if (DB) {
-                        gx[k] += ey[k1] * wv[k2] - ey[k2] * wv[k1];
-                        gy[k] += ex[k2] * wv[k1] - ex[k1] * wv[k2];
-                        gw[k] += ex[k1] * y[k2] - ex[k2] * y[k1] + ey[k2] * x[k1] - ey[k1] * x[k2];
+                        gx += ey[k1] * c.w[k2] - ey[k2] * c.w[k1];
+                        gy += ex[k2] * c.w[k1] - ex[k1] * c.w[k2];
+                        gw += ex[k1] * c.y[k2] - ex[k2] * c.y[k1] + ey[k2] * c.x[k1] - ey[k1] * c.x[k2];
                     }
+                    gv[k][0] = gx; gv[k][1] = gy; gv[k][2] = gw;
                 }
             }
         }
     }
-    // every lane of the warp reaches the match (no early exit above); lanes without a gradient get a key of their own
     const unsigned lane = threadIdx.x & 31u;
-    const long long key = id >= 0 ? (long long)b * p.T + id : -1ll - (long long)lane;
-    const unsigned peers = __match_any_sync(0xFFFFFFFFu, key);
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, id >= 0 ? (long long)b * p.T + id : -1ll - (long long)lane);
     if (id < 0) return;
-    if (peers != (1u << lane)) {
+    bool lead = true;
 #pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            float sx = 0.0f, sy = 0.0f, sw = 0.0f;
-            for (unsigned m = peers; m; m &= m - 1) {
-                const int src = __ffs(m) - 1;
-                sx += __shfl_sync(peers, gx[k], src); sy += __shfl_sync(peers, gy[k], src); sw += __shfl_sync(peers, gw[k], src);
-            }
-            gx[k] = sx; gy[k] = sy; gw[k] = sw;
-        }
-        if ((int)lane != __ffs(peers) - 1) return;
-    }
+    for (int k = 0; k < 3; ++k) lead = warp_group_sum(peers, gv[k]);
+    if (!lead) return;
     float *D = p.dpos + (int64_t)b * p.pos_bs;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
         float *d = D + 4 * (size_t)vi[k];
-        atomicAdd(d, gx[k]); atomicAdd(d + 1, gy[k]); atomicAdd(d + 3, gw[k]);
+        atomicAdd(d, gv[k][0]); atomicAdd(d + 1, gv[k][1]); atomicAdd(d + 3, gv[k][2]);
     }
 }
 
@@ -529,12 +526,10 @@ __device__ __forceinline__ float3 aa_vert(const float *P, int v)
     return make_float3(__ldg(q), __ldg(q + 1), __ldg(q + 3));
 }
 
-// homogeneous edge function a_A x a_B at NDC point (px, py), a = (x - px w, y - py w)
+// homogeneous edge function a_A x a_B at NDC point (px, py)
 __device__ __forceinline__ float aa_edge(float3 A, float3 B, float px, float py)
 {
-    const float ax = __fsub_rn(A.x, __fmul_rn(px, A.z)), ay = __fsub_rn(A.y, __fmul_rn(py, A.z));
-    const float bx = __fsub_rn(B.x, __fmul_rn(px, B.z)), by = __fsub_rn(B.y, __fmul_rn(py, B.z));
-    return __fsub_rn(__fmul_rn(ax, by), __fmul_rn(ay, bx));
+    return clip_edge(clip_a(A.x, A.y, A.z, px, py), clip_a(B.x, B.y, B.z, px, py));
 }
 
 // facing: det[[x0,y0,w0],[x1,y1,w1],[x2,y2,w2]] > 0
@@ -618,7 +613,8 @@ __global__ void __launch_bounds__(256) k_antialias(const AAParams p)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.npx) return;
-    const int ix = (int)(i % p.W); const int64_t t_ = i / p.W; const int iy = (int)(t_ % p.H), b = (int)(t_ / p.H);
+    int b, iy, ix;
+    px_decode(i, p.H, p.W, b, iy, ix);
     const float4 r = __ldg(p.rast + i);
     const int tp = aa_tid(r, p.T);
     const int C = p.C;
@@ -777,14 +773,22 @@ int mcs_interpolate_bwd_rast(const float *attr, int64_t attr_batch_stride, int32
     return 0;
 }
 
+// outs: the entry point's own pointers are present
+static int rast_bwd_common(RastBwdParams &p, const char *name, bool outs, const float *pos, int64_t pos_batch_stride, int32_t V,
+                           const int32_t *tris, int32_t T, const float *rast, int32_t B, int32_t H, int32_t W)
+{
+    MCS_REQUIRE(pos && tris && rast && outs && V > 0 && T > 0 && B > 0 && H > 0 && W > 0 && pos_batch_stride >= 0, "%s: bad arguments", name);
+    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast;
+    p.B = B; p.H = H; p.W = W;
+    return 0;
+}
+
 int mcs_rasterize_bwd(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B, int32_t H,
                       int32_t W, const float *d_rast, float *d_pos, mcs_stream stream)
 {
-    MCS_REQUIRE(pos && tris && rast && d_rast && d_pos && V > 0 && T > 0 && B > 0 && H > 0 && W > 0 && pos_batch_stride >= 0,
-                "mcs_rasterize_bwd: bad arguments");
     RastBwdParams p{};
-    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast; p.drast = (const float4 *)d_rast;
-    p.B = B; p.H = H; p.W = W; p.dpos = d_pos;
+    if (int e = rast_bwd_common(p, "mcs_rasterize_bwd", d_rast && d_pos, pos, pos_batch_stride, V, tris, T, rast, B, H, W)) return e;
+    p.drast = (const float4 *)d_rast; p.dpos = d_pos;
     const int64_t n = (int64_t)B * H * W;
     k_rasterize_bwd<false><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
     MCS_LAUNCH_CHECK();
@@ -794,10 +798,9 @@ int mcs_rasterize_bwd(const float *pos, int64_t pos_batch_stride, int32_t V, con
 int mcs_rast_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B, int32_t H,
                 int32_t W, float *rast_db, mcs_stream stream)
 {
-    MCS_REQUIRE(pos && tris && rast && rast_db && V > 0 && T > 0 && B > 0 && H > 0 && W > 0 && pos_batch_stride >= 0, "mcs_rast_db: bad arguments");
     RastBwdParams p{};
-    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast;
-    p.B = B; p.H = H; p.W = W; p.rast_db = (float4 *)rast_db;
+    if (int e = rast_bwd_common(p, "mcs_rast_db", rast_db != nullptr, pos, pos_batch_stride, V, tris, T, rast, B, H, W)) return e;
+    p.rast_db = (float4 *)rast_db;
     const int64_t n = (int64_t)B * H * W;
     k_rast_db<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
     MCS_LAUNCH_CHECK();
@@ -807,11 +810,9 @@ int mcs_rast_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int
 int mcs_rasterize_bwd_db(const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const float *rast, int32_t B,
                          int32_t H, int32_t W, const float *d_rast, const float *d_rast_db, float *d_pos, mcs_stream stream)
 {
-    MCS_REQUIRE(pos && tris && rast && d_rast_db && d_pos && V > 0 && T > 0 && B > 0 && H > 0 && W > 0 && pos_batch_stride >= 0,
-                "mcs_rasterize_bwd_db: bad arguments");
     RastBwdParams p{};
-    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.rast = (const float4 *)rast; p.drast = (const float4 *)d_rast;
-    p.drast_db = (const float4 *)d_rast_db; p.B = B; p.H = H; p.W = W; p.dpos = d_pos;
+    if (int e = rast_bwd_common(p, "mcs_rasterize_bwd_db", d_rast_db && d_pos, pos, pos_batch_stride, V, tris, T, rast, B, H, W)) return e;
+    p.drast = (const float4 *)d_rast; p.drast_db = (const float4 *)d_rast_db; p.dpos = d_pos;
     const int64_t n = (int64_t)B * H * W;
     k_rasterize_bwd<true><<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(p);
     MCS_LAUNCH_CHECK();

@@ -43,13 +43,6 @@
 // three samples 2.77-2.82 ms against 2.88-3.28 ms for a row of 32 pixels); d tex issues plain vector reductions (1.36-1.46 ms) --
 // grouping the lanes that hit one texel with __match_any_sync costs more than it saves here (2.77-2.82 ms; taps 1.96-1.99 ms against
 // 1.31-1.37 ms).
-// Both alternatives stay buildable for re-measuring with tools/build_variant.sh.
-#ifndef MCS_TEX_AGG
-#define MCS_TEX_AGG 0          // 1 = group lanes of a warp that scatter into the same texel (__match_any_sync)
-#endif
-#ifndef MCS_TEX_TILE
-#define MCS_TEX_TILE 1         // 0 = a row of 32 pixels per warp
-#endif
 
 namespace {
 
@@ -184,32 +177,11 @@ __device__ __forceinline__ float bilerp(float t00, float t10, float t01, float t
     return __fadd_rn(__fmul_rn(oy, top), __fmul_rn(fy, bot));
 }
 
-// d tex of one tap and channel group: one vector reduction (red.global.add.v4/.v2.f32).  With MCS_TEX_AGG, lanes of the warp that scatter
-// into the same texel of the same level sum their values with shuffles (lane order) and one lane issues the reduction; every lane of the
-// warp calls this (live = false for a lane without a gradient).
+// d tex of one tap and channel group: one vector reduction (red.global.add.v4/.v2.f32)
 template <int VEC>
-__device__ __forceinline__ void scatter(float *base, int64_t off, int k, Vec<VEC> g, bool live)
+__device__ __forceinline__ void scatter(float *base, int64_t off, Vec<VEC> g, bool live)
 {
-#if MCS_TEX_AGG
-    const unsigned lane = threadIdx.x & 31u;
-    const uint64_t key = live ? ((uint64_t)off << 4) | (uint64_t)k : (1ull << 63) + lane;
-    const unsigned peers = __match_any_sync(0xFFFFFFFFu, key);
     if (!live) return;
-    if (peers != (1u << lane)) {
-        Vec<VEC> s;
-#pragma unroll
-        for (int j = 0; j < VEC; ++j) s.v[j] = 0.0f;
-        for (unsigned m = peers; m; m &= m - 1) {
-            const int src = __ffs(m) - 1;
-#pragma unroll
-            for (int j = 0; j < VEC; ++j) s.v[j] = __fadd_rn(s.v[j], __shfl_sync(peers, g.v[j], src));
-        }
-        if ((int)lane != __ffs(peers) - 1) return;
-        g = s;
-    }
-#else
-    if (!live) return;
-#endif
     float *p = base + off;
     if (VEC == 4) atomicAdd((float4 *)p, make_float4(g.v[0], g.v[1], g.v[2], g.v[3]));
     else if (VEC == 2) atomicAdd((float2 *)p, make_float2(g.v[0], g.v[1]));
@@ -217,7 +189,7 @@ __device__ __forceinline__ void scatter(float *base, int64_t off, int k, Vec<VEC
 }
 
 template <int VEC>
-__device__ __forceinline__ void scatter_level(float *grad, const Taps &t, int k, int cg, float wl, const Vec<VEC> &g, bool live)
+__device__ __forceinline__ void scatter_level(float *grad, const Taps &t, int cg, float wl, const Vec<VEC> &g, bool live)
 {
     const float ox = __fsub_rn(1.0f, t.fx), oy = __fsub_rn(1.0f, t.fy);
     const float w[4] = {__fmul_rn(wl, __fmul_rn(oy, ox)), __fmul_rn(wl, __fmul_rn(oy, t.fx)), __fmul_rn(wl, __fmul_rn(t.fy, ox)),
@@ -228,15 +200,14 @@ __device__ __forceinline__ void scatter_level(float *grad, const Taps &t, int k,
         Vec<VEC> s;
 #pragma unroll
         for (int i = 0; i < VEC; ++i) s.v[i] = __fmul_rn(w[j], g.v[i]);
-        scatter<VEC>(grad, o[j] + cg, k, s, live);
+        scatter<VEC>(grad, o[j] + cg, s, live);
     }
 }
 
-// pixel of this thread: a row of 32 pixels per warp, or an 8 x 4 tile per warp (MCS_TEX_TILE)
+// pixel of this thread: an 8 x 4 tile per warp
 __device__ __forceinline__ bool tex_pixel(const TexArgs &a, int &b, int &y, int &x, int64_t &pix)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-#if MCS_TEX_TILE
     const int64_t tx = (a.W + 7) / 8, ty = (a.H + 3) / 4, per = tx * ty;
     const int64_t w = i >> 5, lane = i & 31;
     b = (int)(w / per);
@@ -244,14 +215,6 @@ __device__ __forceinline__ bool tex_pixel(const TexArgs &a, int &b, int &y, int 
     y = (int)(t / tx) * 4 + (int)(lane >> 3);
     x = (int)(t % tx) * 8 + (int)(lane & 7);
     const bool in = b < a.B && y < a.H && x < a.W;
-#else
-    const int64_t hw = (int64_t)a.H * a.W;
-    b = (int)(i / hw);
-    const int64_t r = i - (int64_t)b * hw;
-    y = (int)(r / a.W);
-    x = (int)(r - (int64_t)y * a.W);
-    const bool in = i < (int64_t)a.B * hw;
-#endif
     pix = ((int64_t)b * a.H + y) * a.W + x;
     return in;
 }
@@ -356,10 +319,9 @@ __global__ void __launch_bounds__(256) k_texture_bwd(const TexArgs a)
                 }
             }
         }
-        // every lane reaches the scatters (warp-uniform trip count: C is uniform), whether or not it has a gradient
         if (a.want_tex) {
-            scatter_level<VEC>(g0, t0, d.l0, cg, w0, g, live && g0 != nullptr);
-            if (a.mip) scatter_level<VEC>(g1, t1, d.l1, cg, f, g, live && two && g1 != nullptr);
+            scatter_level<VEC>(g0, t0, cg, w0, g, live && g0 != nullptr);
+            if (a.mip) scatter_level<VEC>(g1, t1, cg, f, g, live && two && g1 != nullptr);
         }
     }
     if (!in) return;
@@ -432,11 +394,7 @@ bool aligned_all(const TexArgs &a, int n_levels, uintptr_t mask)
 int tex_launch(const TexArgs &a, cudaStream_t s, bool bwd)
 {
     const int C = a.lv.C;
-#if MCS_TEX_TILE
     const int64_t n_threads = (int64_t)a.B * ((a.W + 7) / 8) * ((a.H + 3) / 4) * 32;
-#else
-    const int64_t n_threads = (int64_t)a.B * a.H * a.W;
-#endif
     const unsigned blocks = (unsigned)((n_threads + 255) / 256);
     const int n = a.lv.n_levels;
     if (C % 4 == 0 && aligned_all(a, n, 15)) { if (bwd) k_texture_bwd<4><<<blocks, 256, 0, s>>>(a); else k_texture_fwd<4><<<blocks, 256, 0, s>>>(a); }

@@ -28,8 +28,6 @@ def _check_pos(pos, B, name):
         raise ValueError("%s: pos must be [V,4] or [B,V,4], got %s" % (name, tuple(pos.shape)))
     if pos.dim() == 3 and pos.shape[0] != B:
         raise ValueError("%s: pos batch %d does not match %d" % (name, pos.shape[0], B))
-    V = pos.shape[-2]
-    return V, (V * 4 if pos.dim() == 3 else 0)
 
 
 def _check_tri(tri, name, what="tri"):
@@ -50,25 +48,6 @@ def _rasterize_launch(optix_ctx, m, resolution, t_state=None):
     return rast
 
 
-class _rasterize_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, pos, tri, optix_ctx, m, resolution, t_state=None):
-        rast = _rasterize_launch(optix_ctx, m, resolution, t_state)
-        ctx.save_for_backward(pos, tri, rast)
-        return rast
-
-    @staticmethod
-    def backward(ctx, d_rast):
-        pos, tri, rast = ctx.saved_tensors
-        B, H, W = rast.shape[0], rast.shape[1], rast.shape[2]
-        d_pos = torch.zeros_like(pos)
-        g = d_rast.to(torch.float32).contiguous()
-        V = pos.shape[-2]
-        L.check(L.lib().mcs_rasterize_bwd(pos.data_ptr(), V * 4 if pos.dim() == 3 else 0, V, tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W,
-                                          g.data_ptr(), d_pos.data_ptr(), L.stream_ptr()), "rasterize (backward)")
-        return d_pos, None, None, None, None, None
-
-
 def _pos_args(pos):
     V = pos.shape[-2]
     return pos.data_ptr(), V * 4 if pos.dim() == 3 else 0, V
@@ -82,21 +61,21 @@ def _rast_db_launch(pos, tri, rast):
     return db
 
 
-class _rasterize_db_func(torch.autograd.Function):
-    """(rast, rast_db) of one rasterize or peel launch; the backward maps d rast and d rast_db to d pos in one launch."""
+class _rasterize_func(torch.autograd.Function):
+    """rast of one rasterize or peel launch, or (rast, rast_db) with grad_db; the backward maps d rast and d rast_db to d pos in one
+    launch."""
     @staticmethod
-    def forward(ctx, pos, tri, optix_ctx, m, resolution, t_state=None):
+    def forward(ctx, pos, tri, optix_ctx, m, resolution, t_state, grad_db):
         ctx.set_materialize_grads(False)
         rast = _rasterize_launch(optix_ctx, m, resolution, t_state)
-        db = _rast_db_launch(pos, tri, rast)
         ctx.save_for_backward(pos, tri, rast)
-        return rast, db
+        return (rast, _rast_db_launch(pos, tri, rast)) if grad_db else rast
 
     @staticmethod
-    def backward(ctx, d_rast, d_db):
+    def backward(ctx, d_rast, d_db=None):
         pos, tri, rast = ctx.saved_tensors
         if not ctx.needs_input_grad[0] or (d_rast is None and d_db is None):
-            return None, None, None, None, None, None
+            return None, None, None, None, None, None, None
         B, H, W = rast.shape[0], rast.shape[1], rast.shape[2]
         d_pos = torch.zeros_like(pos)
         g = d_rast.to(torch.float32).contiguous() if d_rast is not None else None
@@ -108,11 +87,18 @@ class _rasterize_db_func(torch.autograd.Function):
             L.check(L.lib().mcs_rasterize_bwd_db(*_pos_args(pos), tri.data_ptr(), tri.shape[0], rast.data_ptr(), B, H, W,
                                                  g.data_ptr() if g is not None else None, h.data_ptr(), d_pos.data_ptr(), L.stream_ptr()),
                     "rasterize_db (backward)")
-        return d_pos, None, None, None, None, None
+        return d_pos, None, None, None, None, None, None
 
 
-def _rasterize_args(name, mtx, pos, tri):
-    """Validated (contiguous fp32 mtx, pos, tri) of a rasterize-style call; pos and tri are None together."""
+def _rasterize_layer(optix_ctx, m, resolution, pos, tri, t_state, grad_db):
+    """rast, or (rast, rast_db) with grad_db, of one rasterize or peel launch; differentiable with respect to pos when pos is given."""
+    if pos is None:
+        return _rasterize_launch(optix_ctx, m, resolution, t_state)
+    return _rasterize_func.apply(pos, tri, optix_ctx, m, resolution, t_state, grad_db)
+
+
+def _rasterize_args(name, mtx, pos, tri, grad_db):
+    """Validated (contiguous fp32 mtx, pos, tri) of a rasterize-style call; pos and tri are None together, and grad_db needs them."""
     L.require_cuda(mtx)
     if mtx.dim() != 3 or mtx.shape[1:] != (4, 4):
         raise ValueError("%s: mtx must be [B,4,4]" % name)
@@ -120,6 +106,8 @@ def _rasterize_args(name, mtx, pos, tri):
     if pos is None:
         if tri is not None:
             raise ValueError("%s: tri is only used together with pos" % name)
+        if grad_db:
+            raise ValueError("%s: grad_db=True needs pos and tri (the derivatives are those of the clip-space triangle)" % name)
         return m, None, None
     if tri is None:
         raise ValueError("%s: pos needs tri" % name)
@@ -140,14 +128,8 @@ def rasterize(optix_ctx, mtx, resolution, pos=None, tri=None, grad_db=False):
 
     grad_db=True returns (rast, rast_db): rast_db [B,H,W,4] = (du/dX, du/dY, dv/dX, dv/dY) in pixels at each pixel centre, for the
     triangle in rast, from the clip-space triangle (so it needs pos and tri), differentiable with respect to pos."""
-    m, pos, tri = _rasterize_args("rasterize", mtx, pos, tri)
-    if grad_db:
-        if pos is None:
-            raise ValueError("rasterize: grad_db=True needs pos and tri (the derivatives are those of the clip-space triangle)")
-        return _rasterize_db_func.apply(pos, tri, optix_ctx, m, resolution)
-    if pos is None:
-        return _rasterize_launch(optix_ctx, m, resolution)
-    return _rasterize_func.apply(pos, tri, optix_ctx, m, resolution)
+    m, pos, tri = _rasterize_args("rasterize", mtx, pos, tri, grad_db)
+    return _rasterize_layer(optix_ctx, m, resolution, pos, tri, None, bool(grad_db))
 
 
 class DepthPeeler:
@@ -168,9 +150,7 @@ class DepthPeeler:
     `rasterize(grad_db=True)`."""
 
     def __init__(self, optix_ctx, mtx, resolution, pos=None, tri=None, grad_db=False):
-        self._m, self._pos, self._tri = _rasterize_args("DepthPeeler", mtx, pos, tri)
-        if grad_db and self._pos is None:
-            raise ValueError("DepthPeeler: grad_db=True needs pos and tri (the derivatives are those of the clip-space triangle)")
+        self._m, self._pos, self._tri = _rasterize_args("DepthPeeler", mtx, pos, tri, grad_db)
         self._ctx, self._res = optix_ctx, tuple(resolution)
         self._grad_db = bool(grad_db)
         self._state = None
@@ -192,25 +172,17 @@ class DepthPeeler:
             raise RuntimeError("DepthPeeler.rasterize_next_layer: only inside the peeler's `with` block")
         if self._ctx._version != self._version:
             raise RuntimeError("DepthPeeler.rasterize_next_layer: the BVH was rebuilt or refitted since the peeler started")
-        if self._grad_db:
-            return _rasterize_db_func.apply(self._pos, self._tri, self._ctx, self._m, self._res, self._state)
-        if self._pos is None:
-            return _rasterize_launch(self._ctx, self._m, self._res, self._state), None
-        return _rasterize_func.apply(self._pos, self._tri, self._ctx, self._m, self._res, self._state), None
+        out = _rasterize_layer(self._ctx, self._m, self._res, self._pos, self._tri, self._state, self._grad_db)
+        return out if self._grad_db else (out, None)
 
 
 class _interpolate_func(torch.autograd.Function):
     @staticmethod
     def forward(ctx, attr, rast, tri):
-        L.require_cuda(attr, rast, tri)
-        if tri.dtype != torch.int32:
-            raise TypeError("interpolate: tri must be int32 [T,3]")
         a = attr.to(torch.float32).contiguous(); r = rast.to(torch.float32).contiguous(); t = tri.contiguous()
         batched = a.dim() == 3
         V, Cn = a.shape[-2], a.shape[-1]
         B, H, W = r.shape[0], r.shape[1], r.shape[2]
-        if batched and a.shape[0] != B:
-            raise ValueError("interpolate: attribute batch %d does not match rast batch %d" % (a.shape[0], B))
         out = torch.empty(B, H, W, Cn, dtype=torch.float32, device=a.device)
         L.check(L.lib().mcs_interpolate_fwd(a.data_ptr(), V * Cn if batched else 0, V, Cn, t.data_ptr(), t.shape[0], r.data_ptr(), B, H, W,
                                             out.data_ptr(), L.stream_ptr()), "interpolate (forward)")
@@ -295,22 +267,24 @@ def interpolate(attr, rast, tri, rast_db=None, diff_attrs=None):
     needs rast_db [B,H,W,4] (from `rasterize(grad_db=True)` or a `DepthPeeler(grad_db=True)` layer) and is [B,H,W,2n] in nvdiffrast's
     layout: channels 2k and 2k+1 hold (dA/dX, dA/dY) of the k-th selected attribute A, zero where rast has no triangle.  out_da is
     differentiable with respect to attr and rast_db (not rast: it does not depend on the barycentrics).  Semantics: csrc/raster.cu."""
-    if diff_attrs is None:
-        return _interpolate_func.apply(attr, rast, tri), None
-    if rast_db is None:
+    da = diff_attrs is not None
+    if da and rast_db is None:
         raise ValueError("interpolate: diff_attrs needs rast_db")
-    L.require_cuda(attr, rast, tri, rast_db)
+    L.require_cuda(attr, rast, tri, *((rast_db,) if da else ()))
     if tri.dtype != torch.int32:
         raise TypeError("interpolate: tri must be int32 [T,3]")
-    if rast.dim() != 4 or rast.shape[3] != 4:
-        raise ValueError("interpolate: rast must be [B,H,W,4], got %s" % (tuple(rast.shape),))
-    if tuple(rast_db.shape) != tuple(rast.shape):
-        raise ValueError("interpolate: rast_db must be [B,H,W,4] like rast %s, got %s" % (tuple(rast.shape), tuple(rast_db.shape)))
-    if attr.dim() not in (2, 3):
-        raise ValueError("interpolate: attr must be [V,C] or [B,V,C], got %s" % (tuple(attr.shape),))
-    idx = _diff_attr_list(diff_attrs, attr.shape[-1])
+    if da:
+        if rast.dim() != 4 or rast.shape[3] != 4:
+            raise ValueError("interpolate: rast must be [B,H,W,4], got %s" % (tuple(rast.shape),))
+        if tuple(rast_db.shape) != tuple(rast.shape):
+            raise ValueError("interpolate: rast_db must be [B,H,W,4] like rast %s, got %s" % (tuple(rast.shape), tuple(rast_db.shape)))
+        if attr.dim() not in (2, 3):
+            raise ValueError("interpolate: attr must be [V,C] or [B,V,C], got %s" % (tuple(attr.shape),))
+        idx = _diff_attr_list(diff_attrs, attr.shape[-1])
+    if attr.dim() == 3 and attr.shape[0] != rast.shape[0]:
+        raise ValueError("interpolate: attribute batch %d does not match rast batch %d" % (attr.shape[0], rast.shape[0]))
     out = _interpolate_func.apply(attr, rast, tri)
-    return out, _interpolate_da_func.apply(attr, rast_db, rast.detach(), tri, idx)
+    return out, (_interpolate_da_func.apply(attr, rast_db, rast.detach(), tri, idx) if da else None)
 
 
 def antialias_topology(tri):
@@ -328,8 +302,8 @@ def antialias_topology(tri):
 
 
 def _aa_args(color, rast, pos, tri, topology):
-    return (color.data_ptr(), color.shape[3], rast.data_ptr(), rast.shape[0], rast.shape[1], rast.shape[2], pos.data_ptr(),
-            pos.shape[-2] * 4 if pos.dim() == 3 else 0, pos.shape[-2], tri.data_ptr(), tri.shape[0], topology.data_ptr())
+    return (color.data_ptr(), color.shape[3], rast.data_ptr(), rast.shape[0], rast.shape[1], rast.shape[2], *_pos_args(pos), tri.data_ptr(),
+            tri.shape[0], topology.data_ptr())
 
 
 class _antialias_func(torch.autograd.Function):

@@ -2,7 +2,7 @@
 
   * the reference module is imported through tests/refshade.py's `reference_render` (stub nvdiffrast, CPU redirection), unedited;
   * the stub's `dr.interpolate` is replaced by one with nvdiffrast's signature `(attr, rast, tri, rast_db=None, diff_attrs=None)`
-    computing on the fp32 oracle of the derivatives (oracle/raster_db.c: interpolate, out_da), with nvdiffrast's broadcast of a [1,V,C] attribute;
+    computing on the fp32 oracle of the derivatives (oracle/geometry.c: interpolate, out_da), with nvdiffrast's broadcast of a [1,V,C] attribute;
   * `shade` on the imported module is replaced by a function that captures its arguments (render_layer's G-buffer) and returns {};
   * `rast` is the oracle's closest hit (u, v = weights of vertices 0 / 1, z/w, id + 1) of a blob+torus scene seen by two perspective
     views at 24 x 32, and `rast_deriv` the oracle's rast_db of the clip-space vertices.
@@ -89,9 +89,9 @@ def oracle_interpolate(geo):
 
 
 def generate():
-    from oracle.raster_db import raster_db_oracle
+    from oracle.geometry import geometry_oracle
     from refshade import reference_render
-    geo = raster_db_oracle()
+    geo = geometry_oracle()
     v, f, v_tex, uv_idx, mtx = scene()
     pos = np.einsum("bij,vj->bvi", mtx.astype(np.float64), np.concatenate([v, np.ones((v.shape[0], 1), np.float32)], 1)).astype(np.float32)
     rast = oracle_rast(v, f, mtx)

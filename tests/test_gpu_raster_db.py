@@ -8,7 +8,6 @@ import torch
 
 from common import rel_l2
 from oracle.geometry import geometry_oracle
-from oracle.raster_db import raster_db_oracle
 from test_gpu_raster import _scene
 from nvdiffrecmc_b200 import synth
 
@@ -34,7 +33,7 @@ def test_rast_db_bit_identical_on_rasterize_and_peel_layers(dev, batched):
     from nvdiffrecmc_b200.raster import DepthPeeler, rasterize
     ctx, v, f, vt, ft, m, pos = _setup(dev)
     p = pos if batched else pos[0].contiguous()            # [V,4]: one clip-space triangle set for both images (still well defined)
-    o = raster_db_oracle()
+    o = geometry_oracle()
     rast, db = rasterize(ctx, m, RES, p, ft, grad_db=True)
     assert torch.equal(rast, rasterize(ctx, m, RES))
     r = _np(rast)
@@ -59,7 +58,7 @@ def test_out_da_bit_identical(dev, Cn, batched):
     rast, db = rasterize(ctx, m, RES, pos, ft, grad_db=True)
     g = torch.Generator().manual_seed(Cn)
     attr = torch.randn((2, v.shape[0], Cn) if batched else (v.shape[0], Cn), generator=g).to(dev)
-    o = raster_db_oracle()
+    o = geometry_oracle()
     for sel in ("all", [min(2, Cn - 1), 0]):
         out, da = interpolate(attr, rast, ft, rast_db=db, diff_attrs=sel)
         n = Cn if sel == "all" else 2
@@ -91,7 +90,7 @@ def test_ndc_invariant(dev):
 def test_backward(dev):
     from nvdiffrecmc_b200.raster import interpolate, rasterize
     ctx, v, f, vt, ft, m, pos0 = _setup(dev)
-    o = raster_db_oracle()
+    o = geometry_oracle()
     gen = torch.Generator().manual_seed(7)
     # interpolate: d rast_db bit for bit, d attr within 1e-5
     rast, db0 = rasterize(ctx, m, RES, pos0, ft, grad_db=True)
@@ -209,7 +208,7 @@ def test_full_size_bench_mesh(dev):
     pos = ru.xfm_points(vt[None], m).contiguous()
     rast, db = rasterize(ctx, m, res, pos, ft, grad_db=True)
     _, da = interpolate(pos, rast, ft, rast_db=db, diff_attrs="all")
-    o = raster_db_oracle()
+    o = geometry_oracle()
     r = _np(rast)
     assert (r[..., 3] > 0).sum() > 100000
     ref = o.rast_db(_np(pos), f, r)

@@ -6,7 +6,7 @@ import os
 import numpy as np
 import pytest
 
-from oracle.raster_db import raster_db_oracle
+from oracle.geometry import geometry_oracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 S_MIN = 1e-3        # pixels whose |S| (twice the clip-space area term) is below this are excluded from the finite-difference checks
@@ -48,7 +48,7 @@ def _rast_ids(rng, B, H, W, T):
 
 
 def test_rast_db_matches_finite_differences():
-    o = raster_db_oracle(f64=True)
+    o = geometry_oracle(f64=True)
     rng = np.random.default_rng(1)
     T, B, H, W = 6, 1, 9, 13
     pos, tris = _persp_soup(rng, T)
@@ -73,7 +73,7 @@ def test_rast_db_matches_finite_differences():
 
 
 def test_rast_db_affine_is_the_hand_computed_constant():
-    o = raster_db_oracle(f64=True)
+    o = geometry_oracle(f64=True)
     H, W = 5, 11                                        # H != W: a swapped 2/W and 2/H would show
     x0, y0, x1, y1, x2, y2 = -0.6, -0.5, 0.7, -0.2, 0.1, 0.8
     pos = np.array([[x0, y0, 0.3, 1.0], [x1, y1, -0.2, 1.0], [x2, y2, 0.5, 1.0]])
@@ -86,7 +86,7 @@ def test_rast_db_affine_is_the_hand_computed_constant():
 
 @pytest.mark.parametrize("batched", [False, True])
 def test_rast_db_backward_matches_finite_differences(batched):
-    o = raster_db_oracle(f64=True)
+    o = geometry_oracle(f64=True)
     rng = np.random.default_rng(3)
     T, B, H, W = 4, 2, 5, 7
     pos1, tris = _persp_soup(rng, T)
@@ -107,7 +107,7 @@ def test_rast_db_backward_matches_finite_differences(batched):
 
 @pytest.mark.parametrize("diff_attrs", ["all", [2, 0, 2]])
 def test_interpolate_da_adjoint_identity(diff_attrs):
-    o = raster_db_oracle(f64=True)
+    o = geometry_oracle(f64=True)
     rng = np.random.default_rng(4)
     T, B, H, W, Cn = 5, 2, 6, 8, 3
     pos, tris = _persp_soup(rng, T)
@@ -124,7 +124,7 @@ def test_interpolate_da_adjoint_identity(diff_attrs):
 
 
 def test_interpolate_da_of_one_hot_attributes():
-    o = raster_db_oracle()
+    o = geometry_oracle()
     rng = np.random.default_rng(5)
     T, B, H, W = 4, 1, 6, 7
     pos, tris = _persp_soup(rng, T, behind=False)
@@ -143,7 +143,7 @@ def test_interpolate_da_of_one_hot_attributes():
 
 
 def test_zeros_for_background_ids_beyond_T_and_degenerate_triangles():
-    for o in (raster_db_oracle(), raster_db_oracle(f64=True)):
+    for o in (geometry_oracle(), geometry_oracle(f64=True)):
         rng = np.random.default_rng(6)
         T, H, W = 3, 4, 5
         pos, tris = _persp_soup(rng, T, behind=False)
@@ -199,7 +199,7 @@ def test_render_layer_golden_regenerates_bit_identically():
     for k in g.files:
         assert g[k].dtype == d[k].dtype and np.array_equal(g[k], d[k]), k
     # the reference reads channels 2:3 and 3:4 of clip_pos_deriv, i.e. dy_clip/dX and dy_clip/dY under nvdiffrast's layout
-    geo = raster_db_oracle()
+    geo = geometry_oracle()
     da = geo.interpolate_da(d["pos"], d["tris"], d["rast"], d["rast_deriv"])
     clip = geo.interpolate(d["pos"], d["tris"], d["rast"])
     eps = np.float32(1e-5)

@@ -64,7 +64,7 @@ __device__ __forceinline__ RayPre ray_pre(f3 o, f3 d)
 // Depth-peeling separation: the next layer along a ray is the closest hit with t > peel_sep(t_prev), one exactly rounded fp32
 // multiply by 1 + 2^-16 (exact in fp32, about 128 ulp of t).  A plain t > t_prev would return the same surface again where a ray
 // crosses a shared edge: Moeller-Trumbore's closed bounds accept it on both triangles at t values a few ulp apart.  Surfaces closer
-// than this along the ray merge into one layer, as nvdiffrast's peeler drops fragments at equal depth.  tests/peel_oracle.c restates it.
+// than this along the ray merge into one layer, as nvdiffrast's peeler drops fragments at equal depth.  oracle/mcoracle.c restates it.
 __device__ __forceinline__ float peel_sep(float t) { return __fmul_rn(t, 1.0000152587890625f); }
 
 #define MCS_STACK 64

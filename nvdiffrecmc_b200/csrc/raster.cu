@@ -16,6 +16,17 @@
 //                   triangles a few ulp apart, and a plain t > t_prev would return that surface again as a spurious layer.  Surfaces
 //                   closer than 2^-16 t (about 128 ulp) along the ray merge into one layer.  Each layer is an ordinary rast: the
 //                   backward below and antialias take it unchanged.
+//                   There is no far-plane clipping: the search runs along the whole line beyond the near point (t < 1e16), so a surface
+//                   beyond the far plane is returned with z/w > 1.
+//                   Rounding (each step one IEEE round-to-nearest operation; oracle/mcoracle.c orc_invert4 / orc_rasterize restate it and
+//                   the GPU equals that fp32 restatement bit for bit):
+//                     - k_invert4: Gauss-Jordan in fp64, pivot = first row with the largest |a| (strict >), d = 1 / pivot (DIV), pivot
+//                       row *= d (DMUL), other rows a = fma(-f, pivot row, a) (DFMA), each entry rounded to fp32 at the end;
+//                     - pixel centre ((ix + 0.5) / W) * 2 - 1: the * 2 is exact, so FMUL + FADD and FFMA give the same value;
+//                     - mul4: fma(m0, x, fma(m1, y, fma(m2, z, m3 * w))) per row; o = near.xyz / near.w and far.xyz / far.w by IEEE
+//                       division, d = far - o;
+//                     - hit point h = fma(d, t, o) per component, then q = mul4(mtx, h, 1), z/w = q.z / q.w (IEEE division);
+//                     - rast = ((1 - u) - v, u, z/w, id + 1).
 //   k_interpolate : out[b,y,x,:] = u * A[i0] + v * A[i1] + (1 - u - v) * A[i2]; backward scatters into dA with float atomics and, when
 //                   the caller asks for it, writes d rast[...,0:2] = (sum_c g_c (A0_c - A2_c), sum_c g_c (A1_c - A2_c)) (one writer per pixel).
 //
@@ -110,9 +121,9 @@ __global__ void __launch_bounds__(128) k_rasterize(const RasterParams p)
     float a[4], c[4];
     mul4(p.inv + 16 * b, x, y, -1.0f, 1.0f, a);
     mul4(p.inv + 16 * b, x, y, 1.0f, 1.0f, c);
-    const f3 o = F3(a[0] / a[3], a[1] / a[3], a[2] / a[3]);
-    const f3 f = F3(c[0] / c[3], c[1] / c[3], c[2] / c[3]);
-    const f3 d = f - o;
+    const f3 o = F3(__fdiv_rn(a[0], a[3]), __fdiv_rn(a[1], a[3]), __fdiv_rn(a[2], a[3]));
+    const f3 f = F3(__fdiv_rn(c[0], c[3]), __fdiv_rn(c[1], c[3]), __fdiv_rn(c[2], c[3]));
+    const f3 d = F3(__fsub_rn(f.x, o.x), __fsub_rn(f.y, o.y), __fsub_rn(f.z, o.z));
     float t_lo = 0.0f;
     if (p.t_state) {
         const float t_prev = p.t_state[i];
@@ -123,10 +134,10 @@ __global__ void __launch_bounds__(128) k_rasterize(const RasterParams p)
     const int id = bvh_closest(p.bvh, o, d, t_lo, t, u, v);
     float4 out = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     if (id >= 0) {
-        const f3 h = o + d * t;
+        const f3 h = F3(__fmaf_rn(d.x, t, o.x), __fmaf_rn(d.y, t, o.y), __fmaf_rn(d.z, t, o.z));
         float q[4];
         mul4(p.mtx + 16 * b, h.x, h.y, h.z, 1.0f, q);
-        out = make_float4(1.0f - u - v, u, q[2] / q[3], (float)(id + 1));
+        out = make_float4(__fsub_rn(__fsub_rn(1.0f, u), v), u, __fdiv_rn(q[2], q[3]), (float)(id + 1));
     }
     reinterpret_cast<float4 *>(p.rast)[i] = out;
     if (p.t_state) p.t_state[i] = id >= 0 ? t : INFINITY;
@@ -150,7 +161,7 @@ __global__ void k_invert4(const float *__restrict__ m, float *__restrict__ inv, 
         for (int r = 0; r < 4; ++r) {
             if (r == col) continue;
             const double f = a[r][col];
-            for (int c = 0; c < 8; ++c) a[r][c] -= f * a[col][c];
+            for (int c = 0; c < 8; ++c) a[r][c] = __fma_rn(-f, a[col][c], a[r][c]);
         }
     }
     for (int r = 0; r < 4; ++r)

@@ -246,6 +246,13 @@ def _envshade_struct(real):
 
 BSDF_MODES = ["pbr", "diffuse", "white"]     # render/optixutils/ops.py:136
 
+PEEL_SEP = np.float32(1.0 + 2.0 ** -16)
+
+
+def peel_sep(t):
+    """fl32(t * (1 + 2^-16)): the separation between consecutive depth-peel layers along a ray."""
+    return (np.asarray(t, np.float32) * PEEL_SEP).astype(np.float32)
+
 
 class Scene:
     """Triangle soup + canonical LBVH held by the C side."""
@@ -280,11 +287,62 @@ class Scene:
                                     vis.ctypes.data, cnt.ctypes.data)
         return (vis, cnt) if return_counters else vis
 
-    def closest_hit(self, ro, rd):
+    def closest_hit(self, ro, rd, t_after=None):
+        """(tri_id [n] (-1 = miss), tuv [n,3] = (t, u, v)) of the closest hit, ties to the lowest id; with t_after [n], the closest
+        hit with t > sep(t_after) (depth peeling's query; t_after = +inf: a miss)."""
         ro = np.ascontiguousarray(ro, self.orc.dt).reshape(-1, 3); rd = np.ascontiguousarray(rd, self.orc.dt).reshape(-1, 3)
         tid = np.zeros(ro.shape[0], np.int32); tuv = np.zeros((ro.shape[0], 3), self.orc.dt)
-        self.orc.lib.orc_closest_hit(self.h, ro.shape[0], ro.ctypes.data, rd.ctypes.data, tid.ctypes.data, tuv.ctypes.data)
+        if t_after is None:
+            self.orc.lib.orc_closest_hit(self.h, ro.shape[0], ro.ctypes.data, rd.ctypes.data, tid.ctypes.data, tuv.ctypes.data)
+        else:
+            ta = np.ascontiguousarray(t_after, self.orc.dt).reshape(-1)
+            assert ta.shape[0] == ro.shape[0]
+            self.orc.lib.orc_closest_hit_beyond(self.h, ro.shape[0], ro.ctypes.data, rd.ctypes.data, ta.ctypes.data, tid.ctypes.data,
+                                               tuv.ctypes.data)
         return tid, tuv
+
+    def peel(self, ro, rd, layers):
+        """Per-layer (tri_id, tuv) of `layers` successive closest_hit(t_after=) calls, each after the previous layer's t (+inf once a
+        ray has no further hit), as one pixel of raster.DepthPeeler."""
+        ta = np.zeros(np.asarray(ro).reshape(-1, 3).shape[0], self.orc.dt)
+        out = []
+        for _ in range(layers):
+            tid, tuv = self.closest_hit(ro, rd, ta)
+            out.append((tid, tuv))
+            ta = np.where(tid >= 0, tuv[:, 0], np.inf).astype(self.orc.dt)
+        return out
+
+    def all_hits(self, ro, rd):
+        """Sorted (t [k], tri_id [k]) of every triangle one ray hits."""
+        t_all = np.zeros(self.T, self.orc.dt)
+        o = np.ascontiguousarray(ro, self.orc.dt).reshape(3); d = np.ascontiguousarray(rd, self.orc.dt).reshape(3)
+        self.orc.lib.orc_every_hit(self.h, o.ctypes.data, d.ctypes.data, t_all.ctypes.data)
+        ids = np.nonzero(t_all >= 0)[0]
+        order = np.lexsort((ids, t_all[ids]))
+        return t_all[ids][order], ids[order].astype(np.int32)
+
+    def invert4(self, mtx):
+        """k_invert4: [B,4,4] (or [4,4]) -> the inverse of each matrix, Gauss-Jordan in double rounded to `real`."""
+        return self.orc.invert4(mtx)
+
+    def rasterize(self, mtx, res, t_state=None, px=None):
+        """k_rasterize for the clip matrices mtx [B,4,4] at res = (H, W): (rast [B,H,W,4], t_state [B,H,W]).  t_state (the peel state
+        after the previous layer, +inf where exhausted; None: layer 0 / plain rasterize) is not modified; the returned one is the
+        state after this layer.  px: flat indices into [B,H,W] -> rast [n,4] and t_state [n] of those pixels only (t_state, when
+        given, is then the state of those pixels)."""
+        m = np.ascontiguousarray(mtx, self.orc.dt).reshape(-1, 4, 4)
+        B, (H, W) = m.shape[0], res
+        if px is None:
+            n, shape, pp = B * H * W, (B, H, W), None
+        else:
+            pp = np.ascontiguousarray(px, np.int64).reshape(-1)
+            assert pp.size == 0 or (pp.min() >= 0 and pp.max() < B * H * W)
+            n, shape = pp.shape[0], (pp.shape[0],)
+        ts = np.zeros(n, self.orc.dt) if t_state is None else np.array(t_state, self.orc.dt).reshape(-1)
+        assert ts.shape[0] == n
+        rast = np.zeros((n, 4), self.orc.dt)
+        self.orc.lib.orc_rasterize(self.h, B, H, W, m.ctypes.data, n, None if pp is None else pp.ctypes.data, ts.ctypes.data, rast.ctypes.data)
+        return rast.reshape(shape + (4,)), ts.reshape(shape)
 
 
 class Oracle:
@@ -301,6 +359,11 @@ class Oracle:
         self.lib.orc_lbvh_export.argtypes = [C.c_void_p] * 7
         self.lib.orc_visibility.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         self.lib.orc_closest_hit.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        self.lib.orc_closest_hit_beyond.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
+        self.lib.orc_every_hit.argtypes = [C.c_void_p] * 4
+        self.lib.orc_every_hit.restype = C.c_int
+        self.lib.orc_invert4.argtypes = [C.c_int, C.c_void_p, C.c_void_p]
+        self.lib.orc_rasterize.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
         self.lib.orc_env_shade.argtypes = [C.c_void_p]
         self.lib.orc_hash_pcg.restype = C.c_uint32
         self.lib.orc_hash_pcg.argtypes = [C.c_uint32, C.c_uint32]
@@ -332,6 +395,14 @@ class Oracle:
 
     def scene(self, verts, tris):
         return Scene(self, verts, tris)
+
+    def invert4(self, mtx):
+        """k_invert4 (raster.cu): the inverse of each 4x4 matrix of mtx [...,4,4], Gauss-Jordan with partial pivoting in double,
+        rounded to `real` (fp32 build: to float, as the kernel).  A singular matrix gives inf / NaN entries."""
+        m = np.ascontiguousarray(mtx, self.dt)
+        inv = np.zeros_like(m)
+        self.lib.orc_invert4(int(m.size // 16), m.ctypes.data, inv.ctypes.data)
+        return inv
 
     # ------------------------------------------------------------------ elementwise ops
     def _run(self, name, ins, chans, extra, outs_ch, extra_after_ins=True, dout=None, dout_ch=None):

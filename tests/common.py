@@ -98,6 +98,111 @@ def ru_edge_inputs(chans, out_c):
     return ins, dout
 
 
+# ------------------------------------------------------------------------------------------ rasterize: cameras and meshes
+def frustum(l, r, b, t, n, f):
+    """glFrustum: an off-axis (asymmetric) perspective projection."""
+    return np.array([[2 * n / (r - l), 0, (r + l) / (r - l), 0], [0, 2 * n / (t - b), (t + b) / (t - b), 0],
+                     [0, 0, -(f + n) / (f - n), -2 * f * n / (f - n)], [0, 0, -1, 0]], np.float64)
+
+
+def ortho(l, r, b, t, n, f):
+    """glOrtho: clip w is 1 everywhere."""
+    return np.array([[2 / (r - l), 0, 0, -(r + l) / (r - l)], [0, 2 / (t - b), 0, -(t + b) / (t - b)],
+                     [0, 0, -2 / (f - n), -(f + n) / (f - n)], [0, 0, 0, 1]], np.float64)
+
+
+RASTER_CAMERAS = ["persp", "offaxis", "ortho", "wide", "inside", "away", "front", "singular"]
+
+
+def raster_mtx(kind, B, aspect=1.0):
+    """[B,4,4] fp32 clip matrices, a different one per view, around a mesh of radius ~1 at the origin.
+      persp / offaxis / ortho / wide: orbit views through a symmetric, an asymmetric, an orthographic and a 1e-2 .. 1e3 frustum;
+      inside:   the eye at the origin, inside the blob, with the near plane at 0.5, so it cuts the surface;
+      away:     orbit eyes looking away from the mesh (every hit has t < 0);
+      front:    eyes near (0, 0, 3) looking down -z (the `far` mesh's quad lies beyond their far plane);
+      singular: view 0 is all zeros, the others have a zero w row."""
+    out = []
+    for b in range(B):
+        ang, tilt = 0.7 * b + 0.3, -0.4 + 0.15 * b
+        mv = synth.orbit_view(ang, tilt=tilt)
+        if kind == "persp":
+            m = synth.perspective(aspect=aspect, n=0.1, f=10.0).astype(np.float64) @ mv
+        elif kind == "offaxis":
+            m = frustum(-0.03 * aspect, 0.06 * aspect, -0.05, 0.035, 0.1, 10.0) @ mv
+        elif kind == "ortho":
+            m = ortho(-1.4 * aspect, 1.2 * aspect, -1.1, 1.5, 0.5, 6.0) @ mv
+        elif kind == "wide":
+            m = synth.perspective(aspect=aspect, n=1e-2, f=1e3).astype(np.float64) @ mv
+        elif kind == "inside":
+            rot = synth.orbit_view(ang, radius=0.0, tilt=tilt)
+            m = synth.perspective(fovy=1.2, aspect=aspect, n=0.5, f=10.0).astype(np.float64) @ rot
+        elif kind == "away":
+            flip = np.diag([-1.0, 1.0, -1.0, 1.0])                   # a half turn about the eye's own y axis
+            m = synth.perspective(aspect=aspect, n=0.1, f=10.0).astype(np.float64) @ flip @ mv
+        elif kind == "front":                                          # eyes near (0, 0, 3), looking down -z
+            m = synth.perspective(aspect=aspect, n=0.1, f=10.0).astype(np.float64) @ synth.orbit_view(0.05 * b, tilt=0.03 * b)
+        elif kind == "singular":
+            m = synth.perspective(aspect=aspect, n=0.1, f=10.0).astype(np.float64) @ mv
+            m[3] = 0.0
+            if b == 0:
+                m[:] = 0.0
+        else:
+            raise ValueError(kind)
+        out.append(m)
+    return np.stack(out).astype(np.float32)
+
+
+def pixel_grid_mesh(H, W, step=2, z=0.0, tilt=0.0):
+    """A planar grid for the identity clip matrix (orthographic, NDC = world) whose vertices lie exactly on pixel centres, as
+    k_rasterize computes them in fp32, every `step` pixels: rays pass through vertices and along edges, where Moeller-Trumbore's
+    closed bounds accept several triangles at the same t and the lowest id must win.  z = z0 + tilt * x."""
+    xs = ((np.arange(0, W, step, dtype=np.float32) + np.float32(0.5)) / np.float32(W) * np.float32(2) - np.float32(1)).astype(np.float32)
+    ys = ((np.arange(0, H, step, dtype=np.float32) + np.float32(0.5)) / np.float32(H) * np.float32(2) - np.float32(1)).astype(np.float32)
+    X, Y = np.meshgrid(xs, ys, indexing="ij")
+    Z = (np.float32(z) + np.float32(tilt) * X).astype(np.float32)
+    v = np.stack([X, Y, Z], -1).reshape(-1, 3).astype(np.float32)
+    nx, ny = xs.size, ys.size
+    idx = np.arange(nx * ny).reshape(nx, ny)
+    a, b, c, d = idx[:-1, :-1], idx[1:, :-1], idx[1:, 1:], idx[:-1, 1:]
+    f = np.concatenate([np.stack([a, b, c], -1).reshape(-1, 3), np.stack([a, c, d], -1).reshape(-1, 3)]).astype(np.int32)
+    return v, f
+
+
+def raster_mesh(kind):
+    """(verts, tris) of the rasterize test meshes:
+      blob+torus: synth.scene_mesh level 2;  icosphere: closed and convex (exactly two layers);
+      dup:        blob+torus with every triangle twice (exact ties in t) and once more with reversed winding;
+      degenerate: blob+torus with zero-area triangles (repeated and collinear vertices) between the real ones;
+      single:     one triangle (T = 1);
+      far:        blob+torus in front of a large quad 20 units from the orbit eyes, beyond their far plane at 10."""
+    if kind == "blob+torus":
+        return synth.scene_mesh("blob+torus", level=2)
+    if kind == "icosphere":
+        v, f = synth.icosphere(3)
+        return v.astype(np.float32), f.astype(np.int32)
+    v, f = synth.scene_mesh("blob+torus", level=2)
+    if kind == "dup":
+        return v, np.concatenate([f, f, f[:, ::-1]]).astype(np.int32)
+    if kind == "degenerate":
+        rng = np.random.default_rng(4)
+        k = f.shape[0] // 4
+        a = rng.integers(0, v.shape[0], (k, 2))
+        rep = np.stack([a[:, 0], a[:, 0], a[:, 1]], -1)                          # two equal corners
+        mid = ((v[a[:, 0]] + v[a[:, 1]]) * np.float32(0.5)).astype(np.float32)   # a corner on the segment of the other two
+        col = np.stack([a[:, 0], v.shape[0] + np.arange(k), a[:, 1]], -1)
+        pnt = np.repeat(a[:, :1], 3, 1)                                          # a single point
+        bad = np.concatenate([rep, col, pnt])
+        allf = np.concatenate([f, bad])
+        order = rng.permutation(allf.shape[0])
+        return np.concatenate([v, mid]).astype(np.float32), allf[order].astype(np.int32)
+    if kind == "single":
+        return np.array([[-0.9, -0.7, 0.2], [0.8, -0.5, -0.1], [0.1, 0.9, 0.0]], np.float32), np.array([[0, 1, 2]], np.int32)
+    if kind == "far":
+        q = np.array([[-40, -40, -17], [40, -40, -17], [40, 40, -17], [-40, 40, -17]], np.float32)
+        return synth.merge((v, f), (q, np.array([[0, 1, 2], [0, 2, 3]], np.int32)))
+    raise ValueError(kind)
+
+
 # ------------------------------------------------------------------------------------------ BVH builds at given triangle counts
 # Triangle counts where the build changes shape (bvh.cu): 1-4 the tiny view, 5-8 an SAH root that may be a leaf run, 1024 the refit's
 # CTA span, 4096 the radix sort's tile, 16 384 the last SAH size, 65 537 seventeen sort tiles.

@@ -29,6 +29,9 @@
 //                     - rast = ((1 - u) - v, u, z/w, id + 1).
 //   k_interpolate : out[b,y,x,:] = u * A[i0] + v * A[i1] + (1 - u - v) * A[i2]; backward scatters into dA with float atomics and, when
 //                   the caller asks for it, writes d rast[...,0:2] = (sum_c g_c (A0_c - A2_c), sum_c g_c (A1_c - A2_c)) (one writer per pixel).
+//                   Rounding: out = fma(u, A0, fma(v, A1, ((1 - u) - v) A2)); d rast accumulates du = fma(g_c, A0_c - A2_c, du) (likewise dv)
+//                   in channel order from 0.  Both are bit-reproducible and equal the fp32 oracle (orc_interpolate_fwd,
+//                   orc_interpolate_bwd_rast) bit for bit; d attr is an order-dependent float-atomic sum.
 //
 // Geometry gradients (render/render.py:284-291 antialiases every G-buffer layer; geometry/dlmesh.py:75 puts its alpha in the loss):
 //
@@ -85,6 +88,12 @@
 //                     the pair (the left / upper one).  Nothing flows through ids, the facing test or the front test.
 //                     The pair arithmetic uses explicitly rounded operations (no FMA contraction) so that the CPU restatement in
 //                     oracle/geometry.c, compiled with -ffp-contract=off, makes the same discrete decisions.
+//                     Rounding of the outputs with one writer per pixel (both bit-reproducible and equal to the fp32 oracle bit for bit):
+//                       - forward: v = c_p, then per pair p gains, in pair order, v = v + w (c_q - c_p), each operation rounded
+//                         (orc_antialias_fwd);
+//                       - d color: v = g_p, then per pair in pair order v = fma(-w, g_p, v) when p gains and v = fma(w, g_q, v) when q
+//                         gains (orc_antialias_bwd_color); it does not depend on whether d pos is computed.
+//                     d pos is an order-dependent float-atomic sum, within float rounding of the oracle's scatter.
 #include "ctx.h"
 #include "bvh_traverse.cuh"
 
@@ -207,8 +216,8 @@ __global__ void __launch_bounds__(256) k_interpolate(const InterpParams p)
             if (MODE == 2) {
                 const float *A = p.attr + base;
                 const float a2 = __ldg(A + (size_t)i2 * p.C + c);
-                du = fmaf(g, __ldg(A + (size_t)i0 * p.C + c) - a2, du);
-                dv = fmaf(g, __ldg(A + (size_t)i1 * p.C + c) - a2, dv);
+                du = __fmaf_rn(g, __fsub_rn(__ldg(A + (size_t)i0 * p.C + c), a2), du);
+                dv = __fmaf_rn(g, __fsub_rn(__ldg(A + (size_t)i1 * p.C + c), a2), dv);
             }
         }
     }
@@ -684,7 +693,7 @@ __global__ void __launch_bounds__(256) k_antialias(const AAParams p)
         for (int c = 0; c < C; ++c) {
             const float g = __ldg(gp + c);
             float v = g;
-            for (int k = 0; k < n; ++k) v = selfk[k] ? v - wk[k] * g : fmaf(wk[k], __ldg(p.dout + jk[k] * C + c), v);
+            for (int k = 0; k < n; ++k) v = selfk[k] ? __fmaf_rn(-wk[k], g, v) : __fmaf_rn(wk[k], __ldg(p.dout + jk[k] * C + c), v);
             dc[c] = v;
         }
     }

@@ -102,10 +102,10 @@ void orc_interpolate_bwd_rast(int B, int H, int W, int C, int64_t attr_bs, const
         if (id >= 0) {
             const real *A = attr + b * attr_bs;
             const int32_t *tri = tris + 3 * (size_t)id;
-            for (int c = 0; c < C; ++c) {
+            for (int c = 0; c < C; ++c) {             /* fused multiply-adds in channel order, as k_interpolate<2> */
                 const real g = d_out[i * C + c], a2 = A[(size_t)tri[2] * C + c];
-                du += g * (A[(size_t)tri[0] * C + c] - a2);
-                dv += g * (A[(size_t)tri[1] * C + c] - a2);
+                du = R_FMA(g, A[(size_t)tri[0] * C + c] - a2, du);
+                dv = R_FMA(g, A[(size_t)tri[1] * C + c] - a2, dv);
             }
         }
         d_rast[4 * i] = du; d_rast[4 * i + 1] = dv; d_rast[4 * i + 2] = 0; d_rast[4 * i + 3] = 0;
@@ -220,6 +220,24 @@ static int aa_pair(const OrcAA *p, int b, int64_t i, int ix, int iy, int64_t j, 
     return 1;
 }
 
+/* t of the crossing edge of each pixel's right (channel 0) and down (channel 1) pair, NaN where the pair has none; t = 1/2 means no
+ * blend (rule 6).  Lets the tests check that a scene really produces the discrete cases it is built for. */
+void orc_antialias_pair_t(int B, int H, int W, const real *rast, int64_t pos_bs, const real *pos, int T, const int32_t *tris, const int32_t *adj,
+                          real *t_out)
+{
+    const OrcAA p = {B, H, W, 0, 0, T, pos_bs, NULL, rast, pos, tris, adj};
+    for (int64_t i = 0; i < (int64_t)B * H * W; ++i) {
+        const int ix = (int)(i % W), iy = (int)((i / W) % H), b = (int)(i / ((int64_t)W * H));
+        for (int d = 0; d < 2; ++d) {
+            const int jx = ix + (d == 0), jy = iy + (d == 1);
+            real w, fx, fy, ox, oy; int64_t gain, front; AAEdge e;
+            e.t = (real)NAN;                              /* aa_pair leaves e.t unset without a crossing edge */
+            if (jx < W && jy < H) aa_pair(&p, b, i, ix, iy, ((int64_t)b * H + jy) * W + jx, jx, jy, d == 0, &w, &gain, &front, &e, &fx, &fy, &ox, &oy);
+            t_out[2 * i + d] = e.t;
+        }
+    }
+}
+
 static OrcAA aa_make(int B, int H, int W, int C, const real *color, const real *rast, int64_t pos_bs, const real *pos, int T, const int32_t *tris,
                      const int32_t *adj)
 {
@@ -259,7 +277,34 @@ static void aa_edge_grad(const AAEdge *e, real px, real py, real s, real *dA, re
     dB[0] -= s * ay; dB[1] += s * ax; dB[3] += s * (px * ay - py * ax);
 }
 
-/* backward, written as a scatter over the pairs (the kernel gathers): d_color (overwritten) and d_pos (accumulated) */
+/* d_color (overwritten) as the kernel gathers it: start from g_p and walk p's pairs in the order left, right, up, down; a pair p gains
+ * gives v = fma(-w, g_p, v), a pair the neighbour q gains v = fma(w, g_q, v) */
+void orc_antialias_bwd_color(int B, int H, int W, int C, const real *color, const real *rast, int64_t pos_bs, const real *pos, int T,
+                             const int32_t *tris, const int32_t *adj, const real *d_out, real *d_color)
+{
+    const OrcAA p = aa_make(B, H, W, C, color, rast, pos_bs, pos, T, tris, adj);
+#pragma omp parallel for schedule(static)
+    for (int64_t i = 0; i < (int64_t)B * H * W; ++i) {
+        const int ix = (int)(i % W), iy = (int)((i / W) % H), b = (int)(i / ((int64_t)W * H));
+        const int nx[4] = {ix - 1, ix + 1, ix, ix}, ny[4] = {iy, iy, iy - 1, iy + 1};
+        real wk[4]; int64_t jk[4]; int self[4]; int n = 0;
+        for (int d = 0; d < 4; ++d) {
+            if (nx[d] < 0 || nx[d] >= W || ny[d] < 0 || ny[d] >= H) continue;
+            const int64_t j = ((int64_t)b * H + ny[d]) * W + nx[d];
+            real w, fx, fy, ox, oy; int64_t gain, front; AAEdge e;
+            if (aa_pair(&p, b, i, ix, iy, j, nx[d], ny[d], d < 2, &w, &gain, &front, &e, &fx, &fy, &ox, &oy)) { wk[n] = w; jk[n] = j; self[n] = gain == i; ++n; }
+        }
+        for (int c = 0; c < C; ++c) {
+            const real g = d_out[i * C + c];
+            real v = g;
+            for (int k = 0; k < n; ++k) v = self[k] ? R_FMA(-wk[k], g, v) : R_FMA(wk[k], d_out[jk[k] * C + c], v);
+            d_color[i * C + c] = v;
+        }
+    }
+}
+
+/* backward, written as a scatter over the pairs: d_color (overwritten; orc_antialias_bwd_color gathers it in the kernel's order) and
+ * d_pos (accumulated) */
 void orc_antialias_bwd(int B, int H, int W, int C, const real *color, const real *rast, int64_t pos_bs, const real *pos, int T, const int32_t *tris,
                        const int32_t *adj, const real *d_out, real *d_color, real *d_pos)
 {

@@ -108,13 +108,25 @@ class GeometryOracle:
         self.lib.orc_antialias_fwd(*args, C.c_void_p(out.ctypes.data))
         return out
 
-    def antialias_bwd(self, color, rast, pos, tris, d_out, adj=None):
-        """-> (d_color, d_pos)"""
+    def antialias_bwd(self, color, rast, pos, tris, d_out, adj=None, scatter=False):
+        """-> (d_color, d_pos).  d_color is gathered per pixel in the kernel's order (the fp32 build equals k_antialias<true> bit for
+        bit), or with scatter=True accumulated pair by pair; d_pos is always the pair-by-pair scatter."""
         keep, args = self._aa_args(color, rast, pos, tris, adj)
         g = self._a(d_out, keep[0].shape)
         dc = np.zeros_like(keep[0]); dp = np.zeros_like(keep[2])
         self.lib.orc_antialias_bwd(*args, C.c_void_p(g.ctypes.data), C.c_void_p(dc.ctypes.data), C.c_void_p(dp.ctypes.data))
+        if not scatter:
+            self.lib.orc_antialias_bwd_color(*args, C.c_void_p(g.ctypes.data), C.c_void_p(dc.ctypes.data))
         return dc, dp
+
+    def antialias_pair_t(self, rast, pos, tris, adj=None):
+        """[B,H,W,2]: t of the crossing edge of each pixel's right (0) and down (1) pair, NaN where the pair has none (t = 1/2: no blend)."""
+        pos, rast, tris, B, H, W, pbs = self._geo(pos, rast, tris)
+        adj = self.aa_topology(tris) if adj is None else np.ascontiguousarray(adj, np.int32)
+        t = np.zeros((B, H, W, 2), self.dt)
+        self.lib.orc_antialias_pair_t(C.c_int(B), C.c_int(H), C.c_int(W), C.c_void_p(rast.ctypes.data), pbs, C.c_void_p(pos.ctypes.data),
+                                      C.c_int(tris.shape[0]), C.c_void_p(tris.ctypes.data), C.c_void_p(adj.ctypes.data), C.c_void_p(t.ctypes.data))
+        return t
 
     def interpolate(self, attr, tris, rast):
         """out [B,H,W,C] = fma(u, A0, fma(v, A1, (1 - u - v) A2)), 0 without a hit (the kernel's operation order)."""

@@ -111,13 +111,15 @@ def ortho(l, r, b, t, n, f):
                      [0, 0, -2 / (f - n), -(f + n) / (f - n)], [0, 0, 0, 1]], np.float64)
 
 
-RASTER_CAMERAS = ["persp", "offaxis", "ortho", "wide", "inside", "away", "front", "singular"]
+RASTER_CAMERAS = ["persp", "offaxis", "ortho", "wide", "inside", "behind", "away", "front", "singular"]
 
 
 def raster_mtx(kind, B, aspect=1.0):
     """[B,4,4] fp32 clip matrices, a different one per view, around a mesh of radius ~1 at the origin.
       persp / offaxis / ortho / wide: orbit views through a symmetric, an asymmetric, an orthographic and a 1e-2 .. 1e3 frustum;
       inside:   the eye at the origin, inside the blob, with the near plane at 0.5, so it cuts the surface;
+      behind:   the eye at the origin with a 160-degree field of view, so triangles at the image's edge have vertices behind the eye
+                (clip w <= 0);
       away:     orbit eyes looking away from the mesh (every hit has t < 0);
       front:    eyes near (0, 0, 3) looking down -z (the `far` mesh's quad lies beyond their far plane);
       singular: view 0 is all zeros, the others have a zero w row."""
@@ -136,6 +138,9 @@ def raster_mtx(kind, B, aspect=1.0):
         elif kind == "inside":
             rot = synth.orbit_view(ang, radius=0.0, tilt=tilt)
             m = synth.perspective(fovy=1.2, aspect=aspect, n=0.5, f=10.0).astype(np.float64) @ rot
+        elif kind == "behind":
+            rot = synth.orbit_view(ang, radius=0.0, tilt=tilt)
+            m = synth.perspective(fovy=2.8, aspect=aspect, n=0.05, f=10.0).astype(np.float64) @ rot
         elif kind == "away":
             flip = np.diag([-1.0, 1.0, -1.0, 1.0])                   # a half turn about the eye's own y axis
             m = synth.perspective(aspect=aspect, n=0.1, f=10.0).astype(np.float64) @ flip @ mv
@@ -152,12 +157,25 @@ def raster_mtx(kind, B, aspect=1.0):
     return np.stack(out).astype(np.float32)
 
 
-def pixel_grid_mesh(H, W, step=2, z=0.0, tilt=0.0):
+def same_bits(a, b):
+    """bit-for-bit equality of two fp32 arrays (so +0 / -0 and NaN payloads count)"""
+    a, b = np.ascontiguousarray(a, np.float32), np.ascontiguousarray(b, np.float32)
+    return a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
+
+
+def nan_bits(a):
+    """int32 bit patterns, every NaN mapped to one pattern: 'bit-identical' up to the NaN payload."""
+    a = np.where(np.isnan(a), np.float32(np.nan), np.asarray(a, np.float32))
+    return a.view(np.int32)
+
+
+def pixel_grid_mesh(H, W, step=2, z=0.0, tilt=0.0, offset=0.5):
     """A planar grid for the identity clip matrix (orthographic, NDC = world) whose vertices lie exactly on pixel centres, as
     k_rasterize computes them in fp32, every `step` pixels: rays pass through vertices and along edges, where Moeller-Trumbore's
-    closed bounds accept several triangles at the same t and the lowest id must win.  z = z0 + tilt * x."""
-    xs = ((np.arange(0, W, step, dtype=np.float32) + np.float32(0.5)) / np.float32(W) * np.float32(2) - np.float32(1)).astype(np.float32)
-    ys = ((np.arange(0, H, step, dtype=np.float32) + np.float32(0.5)) / np.float32(H) * np.float32(2) - np.float32(1)).astype(np.float32)
+    closed bounds accept several triangles at the same t and the lowest id must win.  z = z0 + tilt * x.  offset = 1 puts the
+    vertices half a pixel further, on pixel corners, so every grid line lies midway between two rows or columns of centres."""
+    xs = ((np.arange(0, W, step, dtype=np.float32) + np.float32(offset)) / np.float32(W) * np.float32(2) - np.float32(1)).astype(np.float32)
+    ys = ((np.arange(0, H, step, dtype=np.float32) + np.float32(offset)) / np.float32(H) * np.float32(2) - np.float32(1)).astype(np.float32)
     X, Y = np.meshgrid(xs, ys, indexing="ij")
     Z = (np.float32(z) + np.float32(tilt) * X).astype(np.float32)
     v = np.stack([X, Y, Z], -1).reshape(-1, 3).astype(np.float32)

@@ -12,14 +12,9 @@ import pytest
 import torch
 
 from common import RU_OPS, env_shade_edge_case, oracle, rel_l2, ru_edge_inputs
+from common import nan_bits as _bits
 
 pytestmark = pytest.mark.gpu
-
-
-def _bits(a):
-    """int32 bit patterns, every NaN mapped to one pattern: 'bit-identical' up to the NaN payload."""
-    a = np.where(np.isnan(a), np.float32(np.nan), np.asarray(a, np.float32))
-    return a.view(np.int32)
 
 
 def _close(got, want, want64, bar, what):

@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from common import oracle, rel_l2
+from common import oracle, rel_l2, same_bits
 from oracle.geometry import geometry_oracle
 from nvdiffrecmc_b200 import synth
 
@@ -157,12 +157,12 @@ def test_gradients_through_peeled_layers(dev):
     args = (color.cpu().numpy(), plain[1], pos0.cpu().numpy(), f)
     ref = o.antialias(*args)
     assert (np.abs(ref - args[0]) > 1e-3).sum() > 50
-    assert rel_l2(out.detach().cpu().numpy(), ref) < 1e-6
+    assert same_bits(out.detach().cpu().numpy(), ref)
     g = torch.randn(out.shape, generator=torch.Generator().manual_seed(11)).to(dev)
     out.backward(g)
     dc, dp = o.antialias_bwd(*args, g.cpu().numpy())
     assert np.abs(dp).max() > 0
-    assert rel_l2(col.grad.cpu().numpy(), dc) < 1e-6 and rel_l2(p.grad.cpu().numpy(), dp) < 1e-5
+    assert same_bits(col.grad.cpu().numpy(), dc) and rel_l2(p.grad.cpu().numpy(), dp) < 1e-5
 
 
 def test_back_to_front_compositing(dev):

@@ -79,8 +79,9 @@ def _view(ang, dist=3.0):
     return _perspective() @ mv
 
 
-def zbuffer(pos, f, H, W):
-    """rast [B,H,W,4] (u, v, z/w, id + 1) of clip-space vertices pos [B,V,4] by brute force (fp64)."""
+def zbuffer(pos, f, H, W, clip_w=True):
+    """rast [B,H,W,4] (u, v, z/w, id + 1) of clip-space vertices pos [B,V,4] by brute force (fp64).  clip_w=False keeps triangles
+    with a vertex at w <= 0, covered where the surface point itself has w > 0 (what a ray from the eye hits)."""
     pos = np.asarray(pos, np.float64)
     B = pos.shape[0]
     px = (np.arange(W) + 0.5) / W * 2 - 1
@@ -91,7 +92,7 @@ def zbuffer(pos, f, H, W):
     for b in range(B):
         for t, tri in enumerate(f):
             q = pos[b, tri]
-            if (q[:, 3] <= 0).any():
+            if clip_w and (q[:, 3] <= 0).any():
                 continue
             ax = q[:, 0][:, None, None] - PX * q[:, 3][:, None, None]
             ay = q[:, 1][:, None, None] - PY * q[:, 3][:, None, None]
@@ -101,8 +102,9 @@ def zbuffer(pos, f, H, W):
                 u, v = s0 / S, s1 / S
                 w2 = 1 - u - v
                 inside = (S != 0) & (u >= 0) & (v >= 0) & (w2 >= 0)
-                zw = (u * q[0, 2] + v * q[1, 2] + w2 * q[2, 2]) / (u * q[0, 3] + v * q[1, 3] + w2 * q[2, 3])
-            m = inside & (zw < depth[b]) & (zw > -1)
+                w = u * q[0, 3] + v * q[1, 3] + w2 * q[2, 3]
+                zw = (u * q[0, 2] + v * q[1, 2] + w2 * q[2, 2]) / w
+            m = inside & (zw < depth[b]) & (zw > -1) & (w > 0)
             depth[b][m] = zw[m]
             rast[b][m] = np.stack([u[m], v[m], zw[m], np.full(m.sum(), t + 1.0)], -1)
     return rast
@@ -178,11 +180,14 @@ def _screen_area(pos, H, W):
     return 0.5 * ((X[1] - X[0]) * (Y[2] - Y[0]) - (X[2] - X[0]) * (Y[1] - Y[0]))
 
 
-def _random_triangle(rng, H, W):
+def _random_triangle(rng, H, W, min_area=0.0):
     while True:
         ndc = rng.uniform(-0.9, 0.9, (3, 2))
         pix = (ndc + 1) * np.array([W, H]) / 2
         if min(np.linalg.norm(pix[k] - pix[(k + 1) % 3]) for k in range(3)) < 100:
+            continue
+        e1, e2 = pix[1] - pix[0], pix[2] - pix[0]
+        if abs(e1[0] * e2[1] - e1[1] * e2[0]) < 2 * min_area:
             continue
         w = rng.uniform(0.5, 2.0, 3)
         z = rng.uniform(-0.5, 0.5, 3) * w
@@ -192,12 +197,34 @@ def _random_triangle(rng, H, W):
 def test_antialias_area_property(geo64):
     """Coverage mask of one large triangle on background, antialiased: the sum is the exact screen area (+-1 % from the one-row
     discretisation per edge) and its gradient the analytic area gradient (+-5 %), over random triangles, perspective w and both windings."""
+    _area_property(geo64, 256, 256)
+
+
+@pytest.mark.parametrize("H,W", [(96, 256), (256, 96)])
+def test_antialias_area_property_non_square(geo64, H, W):
+    """The area property where a pixel step differs in NDC along x and y (triangles of at least 2000 pixels: on a thin one the
+    per-edge discretisation is a larger share of the area)."""
+    _area_property(geo64, H, W, min_area=2000.0)
+
+
+@pytest.mark.parametrize("H,W", [(96, 256), (256, 96)])
+def test_antialias_axis_rule_measures_pixels(geo64, H, W):
+    """Rule 4 measures dX in columns and dY in rows.  Every edge of this triangle has an NDC slope between H/W and W/H, so in pixels
+    it is closer to horizontal than vertical at 96x256 (only vertical pairs cross it) and the other way round at 256x96.  The area
+    property cannot see this: either choice of axis integrates to nearly the same area."""
+    pos = np.array([[-0.6, -0.6, 0.0, 1.0], [0.6, 0.0, 0.0, 1.0], [0.0, 0.7, 0.0, 1.0]])
+    f = np.array([[0, 1, 2]], np.int32)
+    t = geo64.antialias_pair_t(zbuffer(pos[None], f, H, W), pos, f)
+    crossed = np.isfinite(t).reshape(-1, 2).sum(0)
+    assert crossed[0 if H > W else 1] > 100 and crossed[1 if H > W else 0] == 0, crossed
+
+
+def _area_property(geo64, H, W, min_area=0.0):
     rng = np.random.default_rng(7)
-    H = W = 256
     f = np.array([[0, 1, 2]], np.int32)
     errs_a, errs_g = [], []
     for trial in range(8):
-        pos = _random_triangle(rng, H, W)
+        pos = _random_triangle(rng, H, W, min_area)
         if trial % 2:
             pos = pos[[0, 2, 1]]
         rast = zbuffer(pos[None], f, H, W)
@@ -210,3 +237,57 @@ def test_antialias_area_property(geo64):
         errs_g.append(rel_l2(dp, ana))
     assert max(errs_a) < 0.01, errs_a
     assert max(errs_g) < 0.05, errs_g
+
+
+# ------------------------------------------------------------------------------------------------ gather, w <= 0, fp32 d rast
+def test_antialias_gather_equals_scatter_and_is_the_adjoint(geo64):
+    """d color gathered per pixel in the kernel's order equals the pair-by-pair scatter, and <antialias(c), g> = <c, d color>."""
+    pos, f, rast = _scene(B=3, res=32)
+    rng = np.random.default_rng(4)
+    color = rng.random(rast.shape[:3] + (3,))
+    g = rng.standard_normal(color.shape)
+    dc, _ = geo64.antialias_bwd(color, rast, pos, f, g)
+    ds, _ = geo64.antialias_bwd(color, rast, pos, f, g, scatter=True)
+    assert np.abs(dc - g).max() > 1e-3
+    assert np.abs(dc - ds).max() <= 1e-12 * np.abs(ds).max()
+    lhs, rhs = float((geo64.antialias(color, rast, pos, f) * g).sum()), float((color * dc).sum())
+    assert abs(lhs - rhs) <= 1e-12 * abs(lhs)
+
+
+def test_antialias_vertex_behind_the_eye(geo64):
+    """A vertex with w <= 0 under covered pixels: every edge ending at it is skipped (rule 3), so its d pos is exactly 0, and the
+    other vertices' d pos matches finite differences."""
+    pos, f, _ = _scene(B=1, res=24)
+    ids = zbuffer(pos, f, 24, 24)[0, ..., 3].astype(np.int64) - 1
+    used = np.unique(f[ids[ids >= 0]])
+    k = used[len(used) // 2]                                        # a vertex of a visible triangle
+    pos = pos.copy()
+    pos[0, k, 3] = -0.25                                            # behind the eye
+    rast = zbuffer(pos, f, 24, 24, clip_w=False)
+    ids = rast[0, ..., 3].astype(np.int64) - 1
+    assert (f[ids[ids >= 0]] == k).any(-1).sum() > 5                 # covered pixels on triangles that use it
+    rng = np.random.default_rng(5)
+    color = rng.random(rast.shape[:3] + (2,))
+    g = rng.standard_normal(color.shape)
+    adj = geo64.aa_topology(f)
+    _, dp = geo64.antialias_bwd(color, rast, pos, f, g, adj)
+    assert (dp[0, k] == 0).all() and np.abs(dp).max() > 0
+    num = _fd(lambda x: float((geo64.antialias(color, rast, x, f, adj) * g).sum()), pos)
+    assert (num[0, k] == 0).all()
+    assert rel_l2(dp, num) < 1e-6
+
+
+def test_interpolate_bwd_rast_fp32_within_ulps(geo, geo64):
+    """The fp32 d rast (the kernel's fused multiply-adds in channel order) within a few ulp of the fp64 one on the same fp32 inputs."""
+    pos, f, rast = _scene()
+    rast = rast.astype(np.float32)
+    rng = np.random.default_rng(6)
+    for C in (1, 5, 9):
+        attr = rng.uniform(-1, 1, (pos.shape[1], C)).astype(np.float32)
+        g = rng.standard_normal(rast.shape[:3] + (C,)).astype(np.float32)
+        d32, d64 = geo.interpolate_bwd_rast(attr, f, rast, g), geo64.interpolate_bwd_rast(attr, f, rast, g)
+        ids = rast[..., 3].astype(np.int64) - 1
+        A = attr[f[np.maximum(ids, 0)]].astype(np.float64)
+        scale = np.stack([(np.abs(A[..., 0, :] - A[..., 2, :]) * np.abs(g)).sum(-1), (np.abs(A[..., 1, :] - A[..., 2, :]) * np.abs(g)).sum(-1)], -1)
+        assert (np.abs(d32[..., :2] - d64[..., :2]) <= 4 * np.finfo(np.float32).eps * scale).all()
+        assert (d32[ids < 0] == 0).all() and np.abs(d32).max() > 0

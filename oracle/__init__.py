@@ -1,17 +1,18 @@
 """CPU oracle for the nvdiffrecmc hot path -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-Thin numpy/ctypes wrapper around ``oracle/mcoracle.c`` (see that file's header for what it
-restates and how it is pinned).  Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s
-``cpu_baseline`` / ``--impl reference`` legs may import this package; ``nvdiffrecmc_b200`` never
-does.
+numpy/ctypes wrappers around the four C restatements in this directory (see each file's header for what it restates and how it is
+pinned): ``Oracle`` and ``Scene`` here wrap ``mcoracle.c``; ``oracle.geometry``, ``oracle.hashgrid`` and ``oracle.texture`` wrap the C file
+of the same name.  Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import
+this package; ``nvdiffrecmc_b200`` never does.
+
+``build()`` compiles every library twice from the same source: fp32 (the oracle proper, compared with the CUDA kernels) and fp64
+(``f64=True``), used only to validate derivatives and hand-derived adjoints by finite differences.  ``CLib`` is the wrappers' common base:
+it loads one library at one precision with a declared signature for every function the library exports, and ``get(f64)`` returns the one
+shared instance of each (library, precision).
 
 ``build_ref()`` / ``Reference`` compile and drive the reference's OWN raygen source on the CPU (oracle/ref_shim -> oracle/_ref, only
 where /root/reference exists; the built library is git-ignored and travels to the GPU box) -- the check of this restatement
 against the reference itself, and the `--impl reference` arm of bench.py.
-
-Two builds of the same source exist: fp32 (the oracle proper, ``Oracle()``) and fp64
-(``Oracle(f64=True)``), the latter used only to validate the hand-derived adjoints by finite
-differences.
 """
 import ctypes as C
 import os
@@ -21,11 +22,7 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _BUILD = os.path.join(_HERE, "_build")
-_SRC = [os.path.join(_HERE, "mcoracle.c"), os.path.join(_HERE, "detmath.h")]
-
-
-def _lib_path(f64):
-    return os.path.join(_BUILD, "libmcoracle_f64.so" if f64 else "libmcoracle_f32.so")
+LIBS = {"mcoracle": ["mcoracle.c", "detmath.h"], "geometry": ["geometry.c"], "hashgrid": ["hashgrid.c"], "texture": ["texture.c"]}  # source, headers
 
 
 def _cpu_has_fma():
@@ -39,19 +36,76 @@ def _cpu_has_fma():
     return False
 
 
+# -ffp-contract=off is mandatory: the fp32 builds make the CUDA kernels' discrete decisions with the same roundings and reproduce their
+# explicitly rounded operations.  -mfma only turns the explicit fmaf() / fma() calls into one instruction (contraction stays off).
+_CFLAGS = ["-O2", "-ffp-contract=off", "-fopenmp", "-shared", "-fPIC"] + (["-mfma"] if _cpu_has_fma() else [])
+
+
+def _lib_path(name, f64):
+    return os.path.join(_BUILD, "lib%s_%s.so" % (name, "f64" if f64 else "f32"))
+
+
+def _compile(cmd, out, inputs, force=False):
+    """Run the compiler command `cmd` with `-o out` unless `out` is at least as new as every input.  The compiler writes a per-process
+    temporary file that then replaces `out` in one step, so another process (a torchrun rank, a test worker) never loads a half-written
+    library."""
+    if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(s) for s in inputs):
+        return
+    os.makedirs(os.path.dirname(out), exist_ok=True)
+    tmp = "%s.%d.tmp" % (out, os.getpid())
+    subprocess.run(cmd + ["-o", tmp], check=True)
+    os.replace(tmp, out)
+
+
+def _build_lib(name, f64, force=False):
+    srcs = [os.path.join(_HERE, s) for s in LIBS[name]]
+    _compile(["gcc"] + _CFLAGS + (["-DORACLE_F64"] if f64 else []) + [srcs[0], "-lm"], _lib_path(name, f64), srcs, force)
+
+
 def build(force=False):
-    """Compile the C restatement with gcc (fp32 + fp64 variants). -ffp-contract=off is mandatory."""
-    os.makedirs(_BUILD, exist_ok=True)
-    for f64 in (False, True):
-        out = _lib_path(f64)
-        if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(s) for s in _SRC):
-            continue
-        cmd = ["gcc", "-O2", "-ffp-contract=off", "-fopenmp", "-shared", "-fPIC", "-o", out, _SRC[0], "-lm"]
-        if _cpu_has_fma():
-            cmd.insert(2, "-mfma")       # only the explicit fmaf()/fma() calls of mt_eval use it (contraction stays off)
-        if f64:
-            cmd.insert(1, "-DORACLE_F64")
-        subprocess.run(cmd, check=True)
+    """Compile every library of LIBS with gcc, fp32 and fp64 (-DORACLE_F64), into oracle/_build/."""
+    for name in LIBS:
+        for f64 in (False, True):
+            _build_lib(name, f64, force)
+
+
+# A signature table maps every function a library exports to ([argument types], result type) (tests/test_oracle_signatures.py checks
+# the tables against the sources).  REAL is a scalar `real`: c_float in the fp32 build, c_double in the fp64 one.
+REAL = "real"
+_P, _I, _I64 = C.c_void_p, C.c_int, C.c_int64
+
+
+class CLib:
+    """One oracle library at one precision: ``f64``, ``dt`` and ``real`` (the numpy and ctypes types of `real`), ``lib`` (rebuilt if
+    stale, then loaded with every function of ``SIGS`` declared) and ``_a``.  ``get(f64)`` returns the one instance of a class and
+    precision that every caller shares."""
+    LIB, SIGS = None, {}
+    _instances = {}
+
+    def __init__(self, f64=False):
+        self.f64 = f64
+        self.dt, self.real = (np.float64, C.c_double) if f64 else (np.float32, C.c_float)
+        _build_lib(self.LIB, f64)
+        self.lib = C.CDLL(_lib_path(self.LIB, f64))
+        for name, (args, res) in self.SIGS.items():
+            fn = getattr(self.lib, name)          # AttributeError if the library does not export it
+            fn.argtypes = [self.real if a is REAL else a for a in args]
+            fn.restype = res
+        sizeof_real, = [n for n in self.SIGS if n.endswith("_sizeof_real")]      # every library exports one
+        assert getattr(self.lib, sizeof_real)() == C.sizeof(self.real)
+
+    @classmethod
+    def get(cls, f64=False):
+        key = (cls, bool(f64))
+        if key not in CLib._instances:
+            CLib._instances[key] = cls(f64)
+        return CLib._instances[key]
+
+    def _a(self, x, shape=None):
+        x = np.ascontiguousarray(np.asarray(x, dtype=self.dt))
+        if shape is not None:
+            x = np.ascontiguousarray(np.broadcast_to(x, shape))
+        return x
 
 
 # ------------------------------------------------------------------------------------------------
@@ -80,12 +134,9 @@ def build_ref(force=False):
             (_REF_LIB_RU, "ref_renderutils.cpp", {"REF_RU_BSDF": REF_RU_BSDF, "REF_RU_NORMAL": REF_RU_NORMAL, "REF_RU_LOSS": REF_RU_LOSS, "REF_RU_MESH": REF_RU_MESH})]
     for out, shim, macros in jobs:
         srcs = [os.path.join(_SHIM, shim), os.path.join(_SHIM, "optix.h")] + list(macros.values())
-        if not force and os.path.exists(out) and all(os.path.getmtime(out) >= os.path.getmtime(s) for s in srcs):
-            continue
-        os.makedirs(_REF_DIR, exist_ok=True)
         cmd = ["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-fopenmp", "-ffp-contract=off", "-w", "-I" + cuda_inc, "-I" + _SHIM]
         cmd += ["-I" + d for d in sorted({os.path.dirname(v) for v in macros.values()})] + ['-D%s="%s"' % kv for kv in macros.items()]
-        subprocess.run(cmd + [srcs[0], "-o", out], check=True)
+        _compile(cmd + [srcs[0]], out, srcs, force)
     return _REF_LIB
 
 
@@ -345,31 +396,58 @@ class Scene:
         return rast.reshape(shape + (4,)), ts.reshape(shape)
 
 
-class Oracle:
+class Oracle(CLib):
+    LIB = "mcoracle"
+    SIGS = {
+        "orc_lambert_fwd": ([_I] + [_P] * 3, None),
+        "orc_lambert_bwd": ([_I] + [_P] * 5, None),
+        "orc_frostbite_fwd": ([_I] + [_P] * 5, None),
+        "orc_frostbite_bwd": ([_I] + [_P] * 9, None),
+        "orc_fresnel_shlick_fwd": ([_I] + [_P] * 4, None),
+        "orc_fresnel_shlick_bwd": ([_I] + [_P] * 7, None),
+        "orc_ndf_ggx_fwd": ([_I] + [_P] * 3, None),
+        "orc_ndf_ggx_bwd": ([_I] + [_P] * 5, None),
+        "orc_lambda_ggx_fwd": ([_I] + [_P] * 3, None),
+        "orc_lambda_ggx_bwd": ([_I] + [_P] * 5, None),
+        "orc_masking_smith_fwd": ([_I] + [_P] * 4, None),
+        "orc_masking_smith_bwd": ([_I] + [_P] * 7, None),
+        "orc_pbr_specular_fwd": ([_I] + [_P] * 5 + [REAL, _P], None),
+        "orc_pbr_specular_bwd": ([_I] + [_P] * 5 + [REAL] + [_P] * 6, None),
+        "orc_pbr_bsdf_fwd": ([_I] + [_P] * 6 + [REAL, _I, _P], None),
+        "orc_pbr_bsdf_bwd": ([_I] + [_P] * 6 + [REAL, _I] + [_P] * 7, None),
+        "orc_prepare_shading_normal_fwd": ([_I] + [_P] * 6 + [_I, _I, _P], None),
+        "orc_prepare_shading_normal_bwd": ([_I] + [_P] * 6 + [_I, _I] + [_P] * 7, None),
+        "orc_update_pdf": ([_I, _I] + [_P] * 4, None),
+        "orc_rand_pcg": ([_P], C.c_uint32),
+        "orc_hash_pcg": ([C.c_uint32, C.c_uint32], C.c_uint32),
+        "orc_scene_create": ([_P, _I, _P, _I], _P),
+        "orc_scene_destroy": ([_P], None),
+        "orc_lbvh_build": ([_P] * 3, None),
+        "orc_lbvh_export": ([_P] * 7, None),
+        "orc_visibility": ([_P, _I, _I] + [_P] * 4, None),
+        "orc_occluded1": ([_P, _I, _P, _P], _I),
+        "orc_closest_hit": ([_P, _I] + [_P] * 4, None),
+        "orc_closest_hit_beyond": ([_P, _I] + [_P] * 5, None),
+        "orc_every_hit": ([_P] * 4, _I),
+        "orc_invert4": ([_I, _P, _P], None),
+        "orc_rasterize": ([_P, _I, _I, _I, _P, _I64, _P, _P, _P], None),
+        "orc_dirs_to_texels": ([_I] * 3 + [_P] * 2, None),
+        "orc_env_shade": ([_P], None),
+        "orc_bilateral_fwd": ([_I] * 3 + [_P] * 3 + [REAL, _P], None),
+        "orc_bilateral_bwd": ([_I] * 3 + [_P] * 2 + [REAL, _P, _P], None),
+        "orc_det_sincos": ([_I] + [_P] * 3, None),
+        "orc_det_atan2": ([_I] + [_P] * 3, None),
+        "orc_det_acos": ([_I] + [_P] * 2, None),
+        "orc_sizeof_real": ([], _I),
+        "orc_sizeof_envshade": ([], _I),
+        "orc_image_loss_fwd": ([_I, _P, _P, _I, _I, _P], None),
+        "orc_image_loss_bwd": ([_I, _P, _P, _I, _I] + [_P] * 3, None),
+        "orc_xfm_fwd": ([_I] * 3 + [_P, _P, _I, _P], None),
+        "orc_xfm_bwd": ([_I, _I, _P, _P, _I, _P], None),
+    }
+
     def __init__(self, f64=False):
-        build()
-        self.f64 = f64
-        self.dt = np.float64 if f64 else np.float32
-        self.real = C.c_double if f64 else C.c_float
-        self.lib = C.CDLL(_lib_path(f64))
-        self.lib.orc_scene_create.restype = C.c_void_p
-        self.lib.orc_scene_create.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
-        self.lib.orc_lbvh_build.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
-        self.lib.orc_scene_destroy.argtypes = [C.c_void_p]
-        self.lib.orc_lbvh_export.argtypes = [C.c_void_p] * 7
-        self.lib.orc_visibility.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        self.lib.orc_closest_hit.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        self.lib.orc_closest_hit_beyond.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
-        self.lib.orc_every_hit.argtypes = [C.c_void_p] * 4
-        self.lib.orc_every_hit.restype = C.c_int
-        self.lib.orc_invert4.argtypes = [C.c_int, C.c_void_p, C.c_void_p]
-        self.lib.orc_rasterize.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]
-        self.lib.orc_env_shade.argtypes = [C.c_void_p]
-        self.lib.orc_hash_pcg.restype = C.c_uint32
-        self.lib.orc_hash_pcg.argtypes = [C.c_uint32, C.c_uint32]
-        self.lib.orc_rand_pcg.restype = C.c_uint32
-        self.lib.orc_rand_pcg.argtypes = [C.c_void_p]
-        assert self.lib.orc_sizeof_real() == (8 if f64 else 4)
+        super().__init__(f64)
         self._ES = _envshade_struct(self.real)
         assert self.lib.orc_sizeof_envshade() == C.sizeof(self._ES), "struct layout mismatch"
 
@@ -379,12 +457,6 @@ class Oracle:
         initialises (torch has usually loaded it already) and torchrun exports OMP_NUM_THREADS=1.  Returns the size in effect."""
         self.lib.omp_set_num_threads(int(n))
         return int(self.lib.omp_get_max_threads())
-
-    def _a(self, x, shape=None):
-        x = np.ascontiguousarray(np.asarray(x, dtype=self.dt))
-        if shape is not None:
-            x = np.ascontiguousarray(np.broadcast_to(x, shape))
-        return x
 
     def _bc(self, *arrs, chans):
         """Broadcast NHWC arrays over their leading dims (size-1 dims broadcast, tensor.h:32)."""
@@ -411,13 +483,8 @@ class Oracle:
         lead, arrs = self._bc(*allin, chans=allch)
         n = int(np.prod(lead)) if len(lead) else 1
         outs = [np.zeros(lead + (c,), self.dt) for c in outs_ch]
-        args = [C.c_int(n)] + [C.c_void_p(a.ctypes.data) for a in arrs[:len(ins)]]
-        for e in extra:
-            args.append(self.real(e) if isinstance(e, float) else C.c_int(int(e)))
-        if dout is not None:
-            args.append(C.c_void_p(arrs[-1].ctypes.data))
-        args += [C.c_void_p(o.ctypes.data) for o in outs]
-        getattr(self.lib, name)(*args)
+        ptr = lambda arrays: [a.ctypes.data for a in arrays]
+        getattr(self.lib, name)(n, *ptr(arrs[:len(ins)]), *extra, *ptr(arrs[len(ins):] + outs))     # arrs[len(ins):]: dout, if given
         return outs[0] if len(outs) == 1 else tuple(outs)
 
     def lambert(self, nrm, wi):
@@ -488,14 +555,13 @@ class Oracle:
         """Env texel ((y << 16) | x) of each direction, computed exactly as env_shade records it."""
         d = np.ascontiguousarray(dirs, self.dt).reshape(-1, 3)
         out = np.zeros(d.shape[0], np.int32)
-        self.lib.orc_dirs_to_texels(C.c_int(d.shape[0]), C.c_int(Hl), C.c_int(Wl), C.c_void_p(d.ctypes.data), C.c_void_p(out.ctypes.data))
+        self.lib.orc_dirs_to_texels(d.shape[0], Hl, Wl, d.ctypes.data, out.ctypes.data)
         return out.reshape(np.asarray(dirs).shape[:-1])
 
     def update_pdf(self, base):
         base = self._a(base); H, W = base.shape[:2]
         pdf = np.zeros((H, W), self.dt); rows = np.zeros(H, self.dt); cols = np.zeros((H, W), self.dt)
-        self.lib.orc_update_pdf(C.c_int(H), C.c_int(W), C.c_void_p(base.ctypes.data), C.c_void_p(pdf.ctypes.data),
-                                C.c_void_p(rows.ctypes.data), C.c_void_p(cols.ctypes.data))
+        self.lib.orc_update_pdf(H, W, base.ctypes.data, pdf.ctypes.data, rows.ctypes.data, cols.ctypes.data)
         return pdf, rows, cols
 
     # ------------------------------------------------------------------ env shade
@@ -565,16 +631,14 @@ class Oracle:
         col = self._a(col); nrm = self._a(nrm); zdz = self._a(zdz)
         B, H, W = col.shape[:3]
         out = np.zeros((B, H, W, 4), self.dt)
-        self.lib.orc_bilateral_fwd(C.c_int(B), C.c_int(H), C.c_int(W), C.c_void_p(col.ctypes.data), C.c_void_p(nrm.ctypes.data),
-                                   C.c_void_p(zdz.ctypes.data), self.real(sigma), C.c_void_p(out.ctypes.data))
+        self.lib.orc_bilateral_fwd(B, H, W, col.ctypes.data, nrm.ctypes.data, zdz.ctypes.data, sigma, out.ctypes.data)
         return out
 
     def bilateral_bwd(self, nrm, zdz, sigma, out_grad):
         nrm = self._a(nrm); zdz = self._a(zdz); out_grad = self._a(out_grad)
         B, H, W = nrm.shape[:3]
         cg = np.zeros((B, H, W, 3), self.dt)
-        self.lib.orc_bilateral_bwd(C.c_int(B), C.c_int(H), C.c_int(W), C.c_void_p(nrm.ctypes.data), C.c_void_p(zdz.ctypes.data),
-                                   self.real(sigma), C.c_void_p(out_grad.ctypes.data), C.c_void_p(cg.ctypes.data))
+        self.lib.orc_bilateral_bwd(B, H, W, nrm.ctypes.data, zdz.ctypes.data, sigma, out_grad.ctypes.data, cg.ctypes.data)
         return cg
 
     def bilateral_denoiser(self, col, nrm, zdz, sigma):
@@ -589,46 +653,43 @@ class Oracle:
         """renderutils/ops.py:476-498: mean over pixels of mean_c(loss)."""
         lead, (a, b) = self._bc(img, target, chans=[3, 3])
         n = int(np.prod(lead)); px = np.zeros(n, self.dt)
-        self.lib.orc_image_loss_fwd(C.c_int(n), C.c_void_p(a.ctypes.data), C.c_void_p(b.ctypes.data), C.c_int(self._LOSSES[loss]),
-                                    C.c_int(1 if tonemapper == "log_srgb" else 0), C.c_void_p(px.ctypes.data))
+        self.lib.orc_image_loss_fwd(n, a.ctypes.data, b.ctypes.data, self._LOSSES[loss], 1 if tonemapper == "log_srgb" else 0, px.ctypes.data)
         return px.sum(dtype=np.float64) / n
 
     def image_loss_bwd(self, img, target, loss="l1", tonemapper="none", dout=1.0):
         lead, (a, b) = self._bc(img, target, chans=[3, 3])
         n = int(np.prod(lead)); dpx = np.full(n, dout / n, self.dt)
         gi = np.zeros(lead + (3,), self.dt); gt = np.zeros(lead + (3,), self.dt)
-        self.lib.orc_image_loss_bwd(C.c_int(n), C.c_void_p(a.ctypes.data), C.c_void_p(b.ctypes.data), C.c_int(self._LOSSES[loss]),
-                                    C.c_int(1 if tonemapper == "log_srgb" else 0), C.c_void_p(dpx.ctypes.data), C.c_void_p(gi.ctypes.data),
-                                    C.c_void_p(gt.ctypes.data))
+        self.lib.orc_image_loss_bwd(n, a.ctypes.data, b.ctypes.data, self._LOSSES[loss], 1 if tonemapper == "log_srgb" else 0, dpx.ctypes.data,
+                                    gi.ctypes.data, gt.ctypes.data)
         return gi, gt
 
     def xfm(self, points, matrix, is_points=True):
         pts = self._a(points); m = self._a(matrix)
         B, V = m.shape[0], pts.shape[1]
         out = np.zeros((B, V, 4 if is_points else 3), self.dt)
-        self.lib.orc_xfm_fwd(C.c_int(B), C.c_int(pts.shape[0]), C.c_int(V), C.c_void_p(pts.ctypes.data), C.c_void_p(m.ctypes.data), C.c_int(int(is_points)),
-                             C.c_void_p(out.ctypes.data))
+        self.lib.orc_xfm_fwd(B, pts.shape[0], V, pts.ctypes.data, m.ctypes.data, int(is_points), out.ctypes.data)
         return out
 
     def xfm_bwd(self, matrix, dout, is_points=True):
         m = self._a(matrix); g = self._a(dout)
         B, V = g.shape[0], g.shape[1]
         out = np.zeros((B, V, 3), self.dt)
-        self.lib.orc_xfm_bwd(C.c_int(B), C.c_int(V), C.c_void_p(m.ctypes.data), C.c_void_p(g.ctypes.data), C.c_int(int(is_points)), C.c_void_p(out.ctypes.data))
+        self.lib.orc_xfm_bwd(B, V, m.ctypes.data, g.ctypes.data, int(is_points), out.ctypes.data)
         return out
 
     # ------------------------------------------------------------------ det math (fp32 only)
     def det_sincos(self, a):
         a = np.ascontiguousarray(a, np.float32); s = np.zeros_like(a); c = np.zeros_like(a)
-        self.lib.orc_det_sincos(C.c_int(a.size), C.c_void_p(a.ctypes.data), C.c_void_p(s.ctypes.data), C.c_void_p(c.ctypes.data))
+        self.lib.orc_det_sincos(a.size, a.ctypes.data, s.ctypes.data, c.ctypes.data)
         return s, c
 
     def det_atan2(self, y, x):
         y = np.ascontiguousarray(y, np.float32); x = np.ascontiguousarray(x, np.float32); o = np.zeros_like(y)
-        self.lib.orc_det_atan2(C.c_int(y.size), C.c_void_p(y.ctypes.data), C.c_void_p(x.ctypes.data), C.c_void_p(o.ctypes.data))
+        self.lib.orc_det_atan2(y.size, y.ctypes.data, x.ctypes.data, o.ctypes.data)
         return o
 
     def det_acos(self, x):
         x = np.ascontiguousarray(x, np.float32); o = np.zeros_like(x)
-        self.lib.orc_det_acos(C.c_int(x.size), C.c_void_p(x.ctypes.data), C.c_void_p(o.ctypes.data))
+        self.lib.orc_det_acos(x.size, x.ctypes.data, o.ctypes.data)
         return o

@@ -11,14 +11,9 @@ if ROOT not in sys.path:
 
 from nvdiffrecmc_b200 import synth  # noqa: E402
 
-_ORACLE = {}
-
-
 def oracle(f64=False):
     from oracle import Oracle
-    if f64 not in _ORACLE:
-        _ORACLE[f64] = Oracle(f64=f64)
-    return _ORACLE[f64]
+    return Oracle.get(f64)
 
 
 def rel_l2(a, b):

@@ -2,8 +2,9 @@
 import numpy as np
 import pytest
 
+from common import oracle
 from nvdiffrecmc_b200 import synth
-from peel_oracle import PeelScene, sep
+from oracle import peel_sep
 
 
 def _rays(n, seed, v, spread=0.3):
@@ -25,7 +26,7 @@ def _mesh(kind):
 @pytest.mark.parametrize("kind", ["blob+torus", "icosphere"])
 def test_peel_lists_every_surface_once(kind):
     v, f = _mesh(kind)
-    sc = PeelScene(v, f)
+    sc = oracle().scene(v, f)
     ro, rd = _rays(300, 7, v)
     layers = sc.peel(ro, rd, 16)
     assert (layers[-1][0] < 0).all(), "16 layers do not exhaust the scene"
@@ -44,19 +45,19 @@ def test_peel_lists_every_surface_once(kind):
             if int(k) in listed_ids:
                 continue
             before = t_l[t_l <= t]
-            assert before.size > 0 and t <= sep(before[-1]), (i, float(t), int(k))     # merged into the layer just before it
+            assert before.size > 0 and t <= peel_sep(before[-1]), (i, float(t), int(k))     # merged into the layer just before it
         # every layer is the smallest (t, id) beyond the previous layer's separation
         lo = np.float32(0)
         for t, k in listed:
             cand = [(tt, kk) for tt, kk in zip(t_all, id_all) if tt > lo]
             assert min(cand, key=lambda x: (x[0], x[1])) == (t, k)
-            lo = sep(t)
+            lo = peel_sep(t)
     assert depth.max() >= 2 and (depth == 0).any()
 
 
 def test_rays_through_a_closed_sphere_have_two_layers():
     v, f = _mesh("icosphere")
-    sc = PeelScene(v, f)
+    sc = oracle().scene(v, f)
     rng = np.random.default_rng(3)
     n = 2000
     d = rng.normal(size=(n, 3)); d /= np.linalg.norm(d, axis=1, keepdims=True)
@@ -72,7 +73,7 @@ def test_shared_edges_do_not_come_back_as_layers():
     """Rays aimed at the midpoints of an icosphere's edges: Moeller-Trumbore's closed bounds accept many of them on both triangles of
     the edge, a few ulp apart.  The separation merges the pair, so no ray sees more than the two surfaces of the sphere."""
     v, f = _mesh("icosphere")
-    sc = PeelScene(v, f)
+    sc = oracle().scene(v, f)
     e = np.unique(np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), 1), axis=0)
     mid = ((v[e[:, 0]] + v[e[:, 1]]) * np.float32(0.5)).astype(np.float32)
     ro = np.broadcast_to(np.array([1.2, -0.8, 4.0], np.float32), mid.shape).copy()

@@ -57,86 +57,50 @@ def _finite(out, name):
 
 
 # ---------------------------------------------------------------------------------------------
-class _fresnel_shlick_func(torch.autograd.Function):
+class _ew_func(torch.autograd.Function):
+    """mcs_<name>_fwd / mcs_<name>_bwd on the operands `ins`, with `scalars` after the operands in both calls: one output of fwd_ch
+    channels forward, one gradient per operand backward (bwd_ch[i] channels, reduced to the operand's shape)."""
     @staticmethod
-    def forward(ctx, f0, f90, cosTheta):
-        ctx.save_for_backward(f0, f90, cosTheta)
-        return _call("fresnel_shlick_fwd", [f0, f90, cosTheta], [], [3])[0]
+    def forward(ctx, name, scalars, fwd_ch, bwd_ch, *ins):
+        ctx.name, ctx.scalars, ctx.bwd_ch = name, scalars, bwd_ch
+        ctx.save_for_backward(*ins)
+        return _call(name + "_fwd", ins, scalars, [fwd_ch])[0]
 
     @staticmethod
     def backward(ctx, dout):
         ins = ctx.saved_tensors
-        g = _call("fresnel_shlick_bwd", ins, [], [3, 3, 1], dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins))
+        g = _call(ctx.name + "_bwd", ins, ctx.scalars, ctx.bwd_ch, dout=dout)
+        return (None,) * 4 + tuple(_reduce_like(a, b) for a, b in zip(g, ins))
 
 
 def _fresnel_shlick(f0, f90, cosTheta, use_python=False):
     """renderutils/ops.py:89-109"""
-    out = _tb.fresnel_schlick(f0, f90, cosTheta) if use_python else _fresnel_shlick_func.apply(f0, f90, cosTheta)
+    out = _tb.fresnel_schlick(f0, f90, cosTheta) if use_python else _ew_func.apply("fresnel_shlick", (), 3, (3, 3, 1), f0, f90, cosTheta)
     return _finite(out, "_fresnel_shlick")
-
-
-class _ggx2_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, which, alphaSqr, cosTheta):
-        ctx.which = which
-        ctx.save_for_backward(alphaSqr, cosTheta)
-        return _call(which + "_fwd", [alphaSqr, cosTheta], [], [1])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call(ctx.which + "_bwd", ins, [], [1, 1], dout=dout)
-        return (None,) + tuple(_reduce_like(a, b) for a, b in zip(g, ins))
 
 
 def _ndf_ggx(alphaSqr, cosTheta, use_python=False):
     """renderutils/ops.py:112-132"""
-    out = _tb.ndf_ggx(alphaSqr, cosTheta) if use_python else _ggx2_func.apply("ndf_ggx", alphaSqr, cosTheta)
+    out = _tb.ndf_ggx(alphaSqr, cosTheta) if use_python else _ew_func.apply("ndf_ggx", (), 1, (1, 1), alphaSqr, cosTheta)
     return _finite(out, "_ndf_ggx")
 
 
 def _lambda_ggx(alphaSqr, cosTheta, use_python=False):
     """renderutils/ops.py:134-154"""
-    out = _tb.lambda_ggx(alphaSqr, cosTheta) if use_python else _ggx2_func.apply("lambda_ggx", alphaSqr, cosTheta)
+    out = _tb.lambda_ggx(alphaSqr, cosTheta) if use_python else _ew_func.apply("lambda_ggx", (), 1, (1, 1), alphaSqr, cosTheta)
     return _finite(out, "_lambda_ggx")
-
-
-class _masking_smith_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, alphaSqr, cosThetaI, cosThetaO):
-        ctx.save_for_backward(alphaSqr, cosThetaI, cosThetaO)
-        return _call("masking_smith_fwd", [alphaSqr, cosThetaI, cosThetaO], [], [1])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call("masking_smith_bwd", ins, [], [1, 1, 1], dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins))
 
 
 def _masking_smith(alphaSqr, cosThetaI, cosThetaO, use_python=False):
     """renderutils/ops.py:156-176"""
-    out = _tb.masking_smith(alphaSqr, cosThetaI, cosThetaO) if use_python else _masking_smith_func.apply(alphaSqr, cosThetaI, cosThetaO)
+    if use_python:
+        out = _tb.masking_smith(alphaSqr, cosThetaI, cosThetaO)
+    else:
+        out = _ew_func.apply("masking_smith", (), 1, (1, 1, 1), alphaSqr, cosThetaI, cosThetaO)
     return _finite(out, "_masking_smith")
 
 
 # ---------------------------------------------------------------------------------------------
-class _prepare_shading_normal_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng, geom_nrm, two_sided_shading, opengl):
-        ctx.two_sided_shading, ctx.opengl = two_sided_shading, opengl
-        ctx.save_for_backward(pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng, geom_nrm)
-        return _call("prepare_shading_normal_fwd", [pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng, geom_nrm],
-                     [C.c_int32(int(two_sided_shading)), C.c_int32(int(opengl))], [3])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call("prepare_shading_normal_bwd", ins, [C.c_int32(int(ctx.two_sided_shading)), C.c_int32(int(ctx.opengl))], [3] * 6, dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins)) + (None, None)
-
-
 _DEFAULT_PNRM = {}
 
 
@@ -160,82 +124,34 @@ def prepare_shading_normal(pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng,
     if use_python:
         out = _tb.prepare_shading_normal(pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng, geom_nrm, two_sided_shading, opengl)
     else:
-        out = _prepare_shading_normal_func.apply(pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng, geom_nrm, two_sided_shading, opengl)
+        out = _ew_func.apply("prepare_shading_normal", (int(two_sided_shading), int(opengl)), 3, (3,) * 6,
+                             pos, view_pos, perturbed_nrm, smooth_nrm, smooth_tng, geom_nrm)
     return _finite(out, "prepare_shading_normal")
 
 
 # ---------------------------------------------------------------------------------------------
-class _lambert_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, nrm, wi):
-        ctx.save_for_backward(nrm, wi)
-        return _call("lambert_fwd", [nrm, wi], [], [1])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call("lambert_bwd", ins, [], [3, 3], dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins))
-
-
 def lambert(nrm, wi, use_python=False):
     """renderutils/ops.py:244-264 -> [minibatch, height, width, 1]"""
-    out = _tb.lambert(nrm, wi) if use_python else _lambert_func.apply(nrm, wi)
+    out = _tb.lambert(nrm, wi) if use_python else _ew_func.apply("lambert", (), 1, (3, 3), nrm, wi)
     return _finite(out, "lambert")
-
-
-class _frostbite_diffuse_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, nrm, wi, wo, linearRoughness):
-        ctx.save_for_backward(nrm, wi, wo, linearRoughness)
-        return _call("frostbite_fwd", [nrm, wi, wo, linearRoughness], [], [1])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call("frostbite_bwd", ins, [], [3, 3, 3, 1], dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins))
 
 
 def frostbite_diffuse(nrm, wi, wo, linearRoughness, use_python=False):
     """renderutils/ops.py:278-300"""
-    out = _tb.frostbite_diffuse(nrm, wi, wo, linearRoughness) if use_python else _frostbite_diffuse_func.apply(nrm, wi, wo, linearRoughness)
+    if use_python:
+        out = _tb.frostbite_diffuse(nrm, wi, wo, linearRoughness)
+    else:
+        out = _ew_func.apply("frostbite", (), 1, (3, 3, 3, 1), nrm, wi, wo, linearRoughness)
     return _finite(out, "frostbite_diffuse")
-
-
-class _pbr_specular_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, col, nrm, wo, wi, alpha, min_roughness):
-        ctx.save_for_backward(col, nrm, wo, wi, alpha)
-        ctx.min_roughness = min_roughness
-        return _call("pbr_specular_fwd", [col, nrm, wo, wi, alpha], [C.c_float(min_roughness)], [3])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call("pbr_specular_bwd", ins, [C.c_float(ctx.min_roughness)], [3, 3, 3, 3, 1], dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins)) + (None,)
 
 
 def pbr_specular(col, nrm, wo, wi, alpha, min_roughness=0.08, use_python=False):
     """renderutils/ops.py:315-339; alpha is [minibatch, height, width, 1]"""
-    out = _tb.pbr_specular(col, nrm, wo, wi, alpha, min_roughness) if use_python else _pbr_specular_func.apply(col, nrm, wo, wi, alpha, min_roughness)
+    if use_python:
+        out = _tb.pbr_specular(col, nrm, wo, wi, alpha, min_roughness)
+    else:
+        out = _ew_func.apply("pbr_specular", (min_roughness,), 3, (3, 3, 3, 3, 1), col, nrm, wo, wi, alpha)
     return _finite(out, "pbr_specular")
-
-
-class _pbr_bsdf_func(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, kd, arm, pos, nrm, view_pos, light_pos, min_roughness, BSDF):
-        ctx.save_for_backward(kd, arm, pos, nrm, view_pos, light_pos)
-        ctx.min_roughness = min_roughness
-        ctx.BSDF = BSDF
-        return _call("pbr_bsdf_fwd", [kd, arm, pos, nrm, view_pos, light_pos], [C.c_float(min_roughness), C.c_int32(BSDF)], [3])[0]
-
-    @staticmethod
-    def backward(ctx, dout):
-        ins = ctx.saved_tensors
-        g = _call("pbr_bsdf_bwd", ins, [C.c_float(ctx.min_roughness), C.c_int32(ctx.BSDF)], [3] * 6, dout=dout)
-        return tuple(_reduce_like(a, b) for a, b in zip(g, ins)) + (None, None)
 
 
 def pbr_bsdf(kd, arm, pos, nrm, view_pos, light_pos, min_roughness=0.08, bsdf="lambert", use_python=False):
@@ -245,7 +161,7 @@ def pbr_bsdf(kd, arm, pos, nrm, view_pos, light_pos, min_roughness=0.08, bsdf="l
     if use_python:
         out = _tb.pbr_bsdf(kd, arm, pos, nrm, view_pos, light_pos, min_roughness, BSDF)
     else:
-        out = _pbr_bsdf_func.apply(kd, arm, pos, nrm, view_pos, light_pos, min_roughness, BSDF)
+        out = _ew_func.apply("pbr_bsdf", (min_roughness, BSDF), 3, (3,) * 6, kd, arm, pos, nrm, view_pos, light_pos)
     return _finite(out, "pbr_bsdf")
 
 

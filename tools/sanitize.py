@@ -37,7 +37,7 @@ for N in (4, 9):
     rast = rasterize(ctx, (proj @ mv)[None], (24, 24))
     att = t("verts").clone().requires_grad_(True)
     interpolate(att, rast, t("tris"))[0].sum().backward()
-# round 2: records entry point (MODE 2), fused shade tail, texel fetch, device-side seed, and -- with MCS_EW_TMA=1 -- the bulk-copy pipeline
+# round 2: records entry point (MODE 2), fused shade tail, texel fetch, device-side seed
 from nvdiffrecmc_b200.optixutils.ops import env_shade_records, shade_combine
 from nvdiffrecmc_b200.raster import texel_fetch
 env_shade_records(ctx, t("mask"), t("ro"), t("pos"), nrm.detach(), t("view"), t("kd"), t("ks"), t("light"), t("pdf"), t("rows"), t("cols"), t("perms"), n_samples_x=N, rnd_seed=1)
@@ -75,10 +75,5 @@ dat = (torch.randn(2, 9, 11, 4, device=dev) * 0.2).requires_grad_(True)
 texture(torch.rand(2, 5, 7, 3, device=dev, requires_grad=True), uvt, filter_mode="linear", boundary_mode="clamp").sum().backward()
 mipc = [torch.rand(1, max(1, 12 >> k), max(1, 20 >> k), 4, device=dev, requires_grad=True) for k in range(5)]
 texture(mipc[0], uvt, dat, mip=mipc[1:]).sum().backward()
-if os.environ.get("MCS_EW_TMA"):
-    B, H, W = 1, 400, 400          # 160 000 px = 312 tiles of 512 px (>= 2 x 132) + a ragged tail
-    ins = [torch.rand(B, H, W, 3, device=dev).requires_grad_(True) for _ in range(6)]
-    y = ru.pbr_bsdf(*ins); y.sum().backward()
-    n2 = ru.prepare_shading_normal(ins[2], ins[4], ins[0], ins[3], ins[1], ins[5]); n2.sum().backward()
 torch.cuda.synchronize()
 print("sanitize workload ok", float(loss), int(v.sum()), tuple(pts.shape))

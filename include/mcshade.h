@@ -302,6 +302,25 @@ int mcs_hashgrid_fwd(const float *x, int64_t n, const float *params, const mcs_h
 int mcs_hashgrid_bwd(const float *x, int64_t n, const float *params, const mcs_hashgrid_levels *lv, const float *d_out, float *d_params,
                      float *d_x, mcs_stream stream);
 
+/* ---- MLP texture: MLPTexture3D.sample (render/mlptexture.py:86-96) fused, one forward kernel and one backward kernel (plus a d W sum over
+ *      chunks); semantics in csrc/mlptexture.cu.  t [n,3] points, aabb [2,3], min_max [2,channels] (row 0 = lo, row 1 = hi), device fp32,
+ *      contiguous.  params / lv: the hash-grid encoding as mcs_hashgrid_*, with lv->n_levels == 16.  weights: a HOST array of hidden + 1
+ *      device pointers, torch Linear.weight layout [out, in] row-major: weights[l] is [32,32] for l < hidden, weights[hidden] [channels,32];
+ *      hidden in 1..4, channels in 1..8.  out [n,channels] is overwritten.  enc [n,32]: the encoding, written by the forward when non-null
+ *      (needed by the backward) and read by the backward; 16-byte aligned.
+ *      The backward adds into d_params (caller-zeroed, float atomics, 8-byte aligned; may be null), overwrites d_t [n,3] (may be null) and
+ *      overwrites d_weights[l] (d_weights is a HOST array of hidden + 1 device pointers; it or any entry may be null) -- the true gradients,
+ *      at least one requested.  d W is deterministic: chunk partials over MCS_MLPTEX_CHUNK consecutive points are written to `workspace`
+ *      (mcs_mlptex_workspace_bytes(n, hidden, channels) bytes of device memory, 16-byte aligned, contents ignored on entry; needed only for
+ *      d W) and summed in chunk order.  n = 0 is a no-op (d W zeroed).  No host sync, no allocation. */
+#define MCS_MLPTEX_CHUNK 1024
+int64_t mcs_mlptex_workspace_bytes(int64_t n, int32_t hidden, int32_t channels);
+int mcs_mlptex_fwd(const float *t, int64_t n, const float *aabb, const float *min_max, const float *params, const mcs_hashgrid_levels *lv,
+                   int32_t hidden, int32_t channels, const float *const *weights, float *out, float *enc, mcs_stream stream);
+int mcs_mlptex_bwd(const float *t, int64_t n, const float *aabb, const float *min_max, const float *params, const mcs_hashgrid_levels *lv,
+                   int32_t hidden, int32_t channels, const float *const *weights, const float *enc, const float *d_out, float *d_params,
+                   float *d_t, float *const *d_weights, void *workspace, mcs_stream stream);
+
 /* ---- filtered, mip-mapped texture sampling: stands in for nvdiffrast's `dr.texture` in Texture2D.sample and its mip chain's backward
  *      (render/texture.py:27-30,57-68), the regulariser taps (render/render.py:54,75-95) and the probe look-ups (render/light.py:64,76);
  *      semantics in csrc/texture.cu.  The level table is passed by value: level k is ptr[k], [Bt, h[k], w[k], C] fp32 contiguous, with

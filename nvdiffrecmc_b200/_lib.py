@@ -14,7 +14,8 @@ _PKG = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_PKG, "csrc")
 _LIBDIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
-SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu"]
+SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu",
+           "mlptexture.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
@@ -142,6 +143,9 @@ _SIGS = {
     "mcs_antialias_bwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
     "mcs_hashgrid_fwd": ([_P, C.c_int64, _P, _P, _P, _P], C.c_int),
     "mcs_hashgrid_bwd": ([_P, C.c_int64, _P, _P, _P, _P, _P, _P], C.c_int),
+    "mcs_mlptex_workspace_bytes": ([C.c_int64, C.c_int32, C.c_int32], C.c_int64),
+    "mcs_mlptex_fwd": ([_P, C.c_int64] + [_P] * 4 + [C.c_int32, C.c_int32] + [_P] * 4, C.c_int),
+    "mcs_mlptex_bwd": ([_P, C.c_int64] + [_P] * 4 + [C.c_int32, C.c_int32] + [_P] * 8, C.c_int),
     "mcs_texture_fwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P, _P], C.c_int),
     "mcs_texture_bwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P] * 5, C.c_int),
 }
@@ -173,7 +177,7 @@ def lib():
 # and for meshes of 5 to 16 384 triangles the shadow view's clustering and emission.
 LAUNCHES = collections.Counter()
 _KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "rasterize_peel": 2,
-                     "antialias_topology": 2, "hashgrid_bwd_both": 2,
+                     "antialias_topology": 2, "hashgrid_bwd_both": 2, "mlptex_bwd_dw": 2,
                      "texture_fwd": 1, "texture_bwd": 1}
 
 

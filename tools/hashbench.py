@@ -9,8 +9,10 @@ Timed (median of REPS after warm-up):
   fwd            mcs_hashgrid_fwd
   bwd_params     mcs_hashgrid_bwd, d params only (into a zeroed buffer, zeroing outside the timed region)
   bwd_params_dx  mcs_hashgrid_bwd, d params and d x
-  sample         MLPTexture3D.sample's composition twice (normalise, clamp, encode, 3 bias-free Linear + ReLU, sigmoid), forward +
-                 backward: the share of the torch MLP shows whether a fused MLP would pay
+  sample         MLPTexture3D.sample twice (normalise, clamp, encode, 3 bias-free Linear + ReLU, sigmoid), forward + backward, as the
+                 torch composition (encoding kernels + torch MLP) and as the fused drop-in nvdiffrecmc_b200.mlptexture.MLPTexture3D
+                 (csrc/mlptexture.cu), the two arms alternated twice; the encode-only composition for scale
+  sample_no_grad the fused forward alone under torch.no_grad() at 2048^2 points (render_uv's bake at texture_res)
   torch_*        the same encoding written in plain PyTorch (gather + weighted sum, autograd), the comparison arm; its backward (an
                  accumulating index_put of 128 values per point) takes seconds per call, so it is the median of 3
 Prints the card name and power limit, the table bytes touched per point (16 levels x 8 corners x 8 B) and the achieved rate.
@@ -31,6 +33,7 @@ import nvdiffrecmc_b200.optixutils as ou
 from nvdiffrecmc_b200 import _lib as L, synth
 from nvdiffrecmc_b200.raster import rasterize, interpolate
 from nvdiffrecmc_b200.tinycudann import Encoding
+from nvdiffrecmc_b200.mlptexture import MLPTexture3D
 
 dev = torch.device("cuda:0")
 REPS = 25
@@ -149,9 +152,27 @@ def run_size(res, raw_only):
         else:
             a.backward(dy[:n // 2]); b.backward(dy[n // 2:])
 
-    r["sample_fwd_bwd_ms"] = event_ms(step, reps=20, label="sample fwd+bwd")
+    tex = MLPTexture3D(aabb, channels=6, min_max=[lo, hi])
+    with torch.no_grad():
+        tex.encoder.params.copy_(enc.params)
+        for w, m in zip(tex.net.weights(), [m for m in net if isinstance(m, torch.nn.Linear)]):
+            w.copy_(m.weight)
+
+    def fused_step():
+        (tex.sample(pj) * g6[0]).sum().backward()
+        (tex.sample(pp) * g6[1]).sum().backward()
+
+    for rnd in range(2):                 # the two arms alternated, twice
+        r["sample_fwd_bwd_ms_%d" % rnd] = event_ms(step, reps=20, label="sample fwd+bwd, torch MLP (round %d)" % rnd)
+        r["fused_sample_fwd_bwd_ms_%d" % rnd] = event_ms(fused_step, reps=20, label="sample fwd+bwd, fused (round %d)" % rnd)
+    r["sample_fwd_bwd_ms"] = min(r["sample_fwd_bwd_ms_0"], r["sample_fwd_bwd_ms_1"])
+    r["fused_sample_fwd_bwd_ms"] = min(r["fused_sample_fwd_bwd_ms_0"], r["fused_sample_fwd_bwd_ms_1"])
     r["encode_only_fwd_bwd_ms"] = event_ms(lambda: step(False), reps=20, label="encode only fwd+bwd")
     r["mlp_share"] = round(1 - r["encode_only_fwd_bwd_ms"] / r["sample_fwd_bwd_ms"], 3)
+    with torch.no_grad():
+        a_f, a_t = tex.sample(pp), sample(pp)
+    r["fused_vs_torch_out_max_abs"] = float((a_f - a_t).abs().max())
+    del tex
     # plain PyTorch comparison arm: forward, and forward + backward of d params and d x
     lvd = {"n_levels": 16, "dense_mask": enc.levels["dense_mask"], "scale": enc.levels["scale"], "res": enc.levels["res"], "offset": enc.levels["offset"]}
     try:
@@ -182,6 +203,12 @@ if __name__ == "__main__":
     for res in res_list:
         out["2x%dx%d^2" % (B, res)] = run_size(res, raw)
         print(res, json.dumps(out["2x%dx%d^2" % (B, res)]), flush=True)
+    if not raw:
+        # render_uv bakes the texture once at texture_res (2048^2 points), forward only
+        tex = MLPTexture3D(torch.tensor([[0.0] * 3, [1.0] * 3], device=dev), channels=6, min_max=[torch.zeros(6, device=dev), torch.ones(6, device=dev)])
+        q = torch.rand(2048 * 2048, 3, device=dev, generator=torch.Generator(device=dev).manual_seed(2))
+        with torch.no_grad():
+            out["sample_no_grad_2048^2_ms"] = event_ms(lambda: tex.sample(q), reps=20, label="fused sample, no_grad, 2048^2")
     print(json.dumps(out))
     if len(sys.argv) > 1:
         json.dump(out, open(sys.argv[1], "w"), indent=1)

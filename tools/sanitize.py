@@ -68,6 +68,14 @@ enc = Encoding(3, {"otype": "HashGrid", "n_levels": 5, "log2_hashmap_size": 9, "
 xh = (torch.rand(1000, 3, device=dev) * 2 - 0.5).requires_grad_(True)
 enc(xh).sum().backward()
 enc(xh.detach()).sum().backward()
+# fused MLP texture: forward, backward with d texc (points across two d W chunks), backward without d texc, no_grad forward
+from nvdiffrecmc_b200.mlptexture import MLPTexture3D
+mlt = MLPTexture3D(torch.tensor([[-1.0] * 3, [1.0] * 3], device=dev), channels=6, min_max=[torch.zeros(6, device=dev), torch.ones(6, device=dev)])
+tm = (torch.rand(1500, 3, device=dev) * 2.4 - 1.2).requires_grad_(True)
+mlt.sample(tm).sum().backward()
+mlt.sample(tm.detach()).sum().backward()
+with torch.no_grad():
+    mlt.sample(tm)
 # filtered texture look-up: 'linear' / 'clamp' on a per-batch 3-channel texture, 'linear-mipmap-linear' / 'wrap' on a custom 4-channel chain
 from nvdiffrecmc_b200.raster import texture
 uvt = (torch.rand(2, 9, 11, 2, device=dev) * 1.6 - 0.3).requires_grad_(True)

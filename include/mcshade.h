@@ -206,7 +206,9 @@ int mcs_xfm_bwd(const mcs_tensor *points, const mcs_tensor *matrix, const mcs_te
 /* ---- tail of render.shade() (row f3): normalise the denoiser outputs and recombine the demodulated signals, render/render.py:119-131.
  *      a4 / b4: [B,H,W,4] raw bilateral outputs (rgb weighted sum, weight) of the diffuse / specular signal; kd, ks [B,H,W,3];
  *      pbr != 0: out = a.rgb/a.w * kd * (1 - ks.z) + b.rgb/b.w ;  pbr == 0 ('diffuse' / 'white'): out = a.rgb/a.w * kd (b4, ks ignored but
- *      must be valid views).  Backward writes contiguous gradients for a4, kd (and b4, ks when pbr). */
+ *      must be valid views).  Backward writes contiguous gradients for a4, kd (and b4, ks when pbr).  Every output has a4's [B,H,W], so
+ *      a4 (and b4 when pbr) must span the broadcast grid of all operands (d_out included); kd / ks / d_out may broadcast.  An a4 / b4
+ *      smaller than that grid is an error, reported before any launch. */
 int mcs_shade_combine_fwd(const mcs_tensor *a4, const mcs_tensor *b4, const mcs_tensor *kd, const mcs_tensor *ks, int32_t pbr, float *out, mcs_stream s);
 int mcs_shade_combine_bwd(const mcs_tensor *a4, const mcs_tensor *b4, const mcs_tensor *kd, const mcs_tensor *ks, int32_t pbr, const mcs_tensor *d_out,
                           float *d_a4, float *d_b4, float *d_kd, float *d_ks, mcs_stream s);

@@ -450,6 +450,24 @@ static int ew(const char *entry, mcs_stream s, Op &op, const Operand (&ins)[N])
     return 0;
 }
 
+// shade_combine writes its outputs at a4's [N,H,W] (and d_b4 at b4's in 'pbr') while ew() launches over the broadcast grid of every
+// operand: an output operand that spans less than that grid would let the kernel write past the end of its buffers.
+template <size_t N>
+static bool spans_grid(const char *entry, const mcs_tensor *t, const char *name, const mcs_tensor *const (&all)[N])
+{
+    if (!view_ok(t)) return true;                     // ew() reports null / empty operands
+    for (const mcs_tensor *o : all) {
+        if (!view_ok(o)) continue;
+        for (int d = 0; d < 3; ++d)
+            if (o->sizes[d] > t->sizes[d]) {
+                mcs_set_error("%s: %s must span the operands' grid (dim %d is %d, another operand has %d): the outputs take its shape",
+                              entry, name, d, t->sizes[d], o->sizes[d]);
+                return false;
+            }
+    }
+    return true;
+}
+
 }  // namespace
 
 extern "C" {
@@ -574,12 +592,16 @@ int mcs_prepare_shading_normal_bwd(const mcs_tensor *pos, const mcs_tensor *view
 
 int mcs_shade_combine_fwd(const mcs_tensor *a4, const mcs_tensor *b4, const mcs_tensor *kd, const mcs_tensor *ks, int32_t pbr, float *out, mcs_stream s)
 {
+    const mcs_tensor *all[] = {a4, b4, kd, ks};
+    if (!spans_grid(__func__, a4, "a4", all) || (pbr && !spans_grid(__func__, b4, "b4", all))) return 1;
     CombineFwd op; op.pbr = pbr; op.out = out;
     return ew(__func__, s, op, {{&op.a4, a4, 4, "a4"}, {&op.b4, b4, 4, "b4"}, {&op.kd, kd, 3, "kd"}, {&op.ks, ks, 3, "ks"}});
 }
 int mcs_shade_combine_bwd(const mcs_tensor *a4, const mcs_tensor *b4, const mcs_tensor *kd, const mcs_tensor *ks, int32_t pbr, const mcs_tensor *d_out,
                           float *d_a4, float *d_b4, float *d_kd, float *d_ks, mcs_stream s)
 {
+    const mcs_tensor *all[] = {a4, b4, kd, ks, d_out};
+    if (!spans_grid(__func__, a4, "a4", all) || (pbr && !spans_grid(__func__, b4, "b4", all))) return 1;
     CombineBwd op; op.pbr = pbr; op.d_a4 = d_a4; op.d_b4 = d_b4; op.d_kd = d_kd; op.d_ks = d_ks;
     return ew(__func__, s, op, {{&op.a4, a4, 4, "a4"}, {&op.b4, b4, 4, "b4"}, {&op.kd, kd, 3, "kd"}, {&op.ks, ks, 3, "ks"},
                                 {&op.dout, d_out, 3, "d_out"}});

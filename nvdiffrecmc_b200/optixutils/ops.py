@@ -362,6 +362,11 @@ class _shade_combine_func(torch.autograd.Function):
     def forward(ctx, a4, b4, kd, ks, pbr):
         L.require_cuda(a4, b4, kd, ks)
         a4, b4, kd, ks = _f32(a4, "a4"), _f32(b4, "b4"), _f32(kd, "kd"), _f32(ks, "ks")
+        # the outputs (and the gradients of a4 / b4) take a4's [B,H,W]; the kernel runs over the broadcast grid of all four operands
+        grid = tuple(max(t.shape[d] for t in (a4, b4, kd, ks)) for d in range(3))
+        for t, name in ((a4, "a4"), (b4, "b4"))[:2 if pbr else 1]:
+            if tuple(t.shape[:3]) != grid:
+                raise RuntimeError("shade_combine: %s %s must span the operands' grid %s" % (name, tuple(t.shape), grid))
         ctx.save_for_backward(a4, b4, kd, ks)
         ctx.pbr = int(pbr)
         out = torch.empty(*a4.shape[:3], 3, dtype=torch.float32, device=a4.device)

@@ -442,6 +442,8 @@ class Oracle(CLib):
         "orc_sizeof_envshade": ([], _I),
         "orc_image_loss_fwd": ([_I, _P, _P, _I, _I, _P], None),
         "orc_image_loss_bwd": ([_I, _P, _P, _I, _I] + [_P] * 3, None),
+        "orc_shade_combine_fwd": ([_I] + [_P] * 4 + [_I, _P], None),
+        "orc_shade_combine_bwd": ([_I] + [_P] * 4 + [_I] + [_P] * 5, None),
         "orc_xfm_fwd": ([_I] * 3 + [_P, _P, _I, _P], None),
         "orc_xfm_bwd": ([_I, _I, _P, _P, _I, _P], None),
     }
@@ -649,20 +651,51 @@ class Oracle(CLib):
     # ------------------------------------------------------------------ row f3: image loss, xfm
     _LOSSES = {"l1": 0, "mse": 1, "relmse": 2, "smape": 3, "n2n": 4}
 
-    def image_loss(self, img, target, loss="l1", tonemapper="none"):
-        """renderutils/ops.py:476-498: mean over pixels of mean_c(loss)."""
+    def image_loss_px(self, img, target, loss="l1", tonemapper="none"):
+        """The per-pixel loss mean_c(loss) of loss.cu:105-141 on the broadcast grid of img and target: [N,H,W]."""
         lead, (a, b) = self._bc(img, target, chans=[3, 3])
         n = int(np.prod(lead)); px = np.zeros(n, self.dt)
         self.lib.orc_image_loss_fwd(n, a.ctypes.data, b.ctypes.data, self._LOSSES[loss], 1 if tonemapper == "log_srgb" else 0, px.ctypes.data)
-        return px.sum(dtype=np.float64) / n
+        return px.reshape(lead)
+
+    @staticmethod
+    def _img_pixels(img):
+        s = np.shape(img)
+        return int(s[0] * s[1] * s[2])
+
+    def image_loss(self, img, target, loss="l1", tonemapper="none"):
+        """renderutils/ops.py:476-498: the per-pixel losses summed over the broadcast grid, divided by IMG's pixel count N*H*W, as
+        renderutils/ops.py:494 divides by img.shape[0:3].  So where img broadcasts against a batched target (img [1,H,W,3], target
+        [N,H,W,3]) the result is N times the mean per-pixel loss, as in the reference and the product."""
+        return self.image_loss_px(img, target, loss, tonemapper).sum(dtype=np.float64) / self._img_pixels(img)
 
     def image_loss_bwd(self, img, target, loss="l1", tonemapper="none", dout=1.0):
+        """Full-grid [N,H,W,3] gradients (img_grad, target_grad).  dout: a scalar, the upstream gradient of image_loss() (so every pixel
+        gets dout / img's pixel count, the divisor rule of image_loss), or an [N,H,W] array, the upstream gradient of each pixel of
+        image_loss_px()."""
         lead, (a, b) = self._bc(img, target, chans=[3, 3])
-        n = int(np.prod(lead)); dpx = np.full(n, dout / n, self.dt)
+        n = int(np.prod(lead))
+        if np.ndim(dout) == 0:
+            dpx = np.full(n, dout / self._img_pixels(img), self.dt)
+        else:
+            dpx = np.ascontiguousarray(np.broadcast_to(np.asarray(dout, self.dt), lead)).reshape(n)
         gi = np.zeros(lead + (3,), self.dt); gt = np.zeros(lead + (3,), self.dt)
         self.lib.orc_image_loss_bwd(n, a.ctypes.data, b.ctypes.data, self._LOSSES[loss], 1 if tonemapper == "log_srgb" else 0, dpx.ctypes.data,
                                     gi.ctypes.data, gt.ctypes.data)
         return gi, gt
+
+    def shade_combine(self, a4, b4, kd, ks, pbr=True):
+        """orc_shade_combine_fwd: the tail of render.shade() (render.py:119-127) on the raw denoiser outputs a4 / b4 [...,4] (rgb weighted
+        sum, weight) -> [...,3].  pbr=False: 'diffuse' / 'white', b4 and ks unused (None allowed)."""
+        b4 = a4 if b4 is None else b4
+        ks = kd if ks is None else ks
+        return self._run("orc_shade_combine_fwd", [a4, b4, kd, ks], [4, 4, 3, 3], [int(pbr)], [3])
+
+    def shade_combine_bwd(self, a4, b4, kd, ks, dout, pbr=True):
+        """-> full-grid (d_a4, d_b4, d_kd, d_ks); d_b4 / d_ks are zero when pbr=False."""
+        b4 = a4 if b4 is None else b4
+        ks = kd if ks is None else ks
+        return self._run("orc_shade_combine_bwd", [a4, b4, kd, ks], [4, 4, 3, 3], [int(pbr)], [4, 4, 3, 3], dout=dout, dout_ch=3)
 
     def xfm(self, points, matrix, is_points=True):
         pts = self._a(points); m = self._a(matrix)

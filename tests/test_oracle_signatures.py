@@ -12,7 +12,7 @@ from oracle.hashgrid import HashGridOracle
 from oracle.texture import TextureOracle
 
 ORACLE_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
-WRAPPERS = [(Oracle, 45), (GeometryOracle, 14), (HashGridOracle, 4), (TextureOracle, 4)]     # exports of each library at the time of writing
+WRAPPERS = [(Oracle, 47), (GeometryOracle, 14), (HashGridOracle, 4), (TextureOracle, 4)]     # exports of each library at the time of writing
 
 
 def _exports(source):

@@ -25,6 +25,12 @@ for N in (4, 9):
     ou.optix_build_bvh(ctx, t("verts"), t("tris"), 0)
     v = ou.trace_visibility(ctx, t("ro").reshape(-1, 3), torch.nn.functional.normalize(torch.randn(c["ro"].size // 3, 3, device=dev), dim=-1))
     pts = ru.xfm_points(t("verts")[None], torch.rand(2, 4, 4, device=dev))
+    # strided operands: channel-strided points, a transposed matrix, a stride-0 upstream gradient; per-partial weighted loss backward
+    ps = t("verts").t().contiguous()[None].transpose(1, 2).requires_grad_(True)
+    ru.xfm_vectors(ps, torch.rand(2, 4, 4, device=dev).transpose(1, 2)).backward(torch.rand(1, ps.shape[1], 3, device=dev).expand(2, -1, 3))
+    from nvdiffrecmc_b200.renderutils.ops import _image_loss_func
+    parts = _image_loss_func.apply(torch.rand(2, 12, 12, 4, device=dev, requires_grad=True)[..., :3], torch.rand(1, 12, 12, 3, device=dev), "relmse", "log_srgb")
+    (parts * torch.rand_like(parts)).sum().backward()
     # re-tracing backward (decorrelated seeds), update_pdf, rasterize / interpolate
     d2, s2 = ou.optix_env_shade(ctx, t("mask"), t("ro"), pos, nrm.detach().requires_grad_(True), t("view"), kd, ks, light, t("pdf"), t("rows"), t("cols"), n_samples_x=N, rnd_seed=None,
                                 perms=t("perms"))

@@ -3,6 +3,8 @@ import ctypes
 import os
 import re
 
+import pytest
+
 from nvdiffrecmc_b200 import _lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -76,3 +78,68 @@ def test_argument_validation_returns_status_and_message():
         msg = l.mcs_last_error() or b""
         assert rc != 0, name
         assert frag in msg, (name, msg)
+
+
+# The renderutils streaming ops: operands (name, channels), the forward output's channel count and the scalar arguments.
+# The backward takes the operands, the scalars and d_out, and writes one gradient per operand.
+EW_OPS = {
+    "lambert": ([("nrm", 3), ("wi", 3)], 1, []),
+    "frostbite": ([("nrm", 3), ("wi", 3), ("wo", 3), ("lin_rough", 1)], 1, []),
+    "fresnel_shlick": ([("f0", 3), ("f90", 3), ("cos_theta", 1)], 3, []),
+    "ndf_ggx": ([("alpha_sqr", 1), ("cos_theta", 1)], 1, []),
+    "lambda_ggx": ([("alpha_sqr", 1), ("cos_theta", 1)], 1, []),
+    "masking_smith": ([("alpha_sqr", 1), ("cos_i", 1), ("cos_o", 1)], 1, []),
+    "pbr_specular": ([("col", 3), ("nrm", 3), ("wo", 3), ("wi", 3), ("alpha", 1)], 3, [0.08]),
+    "pbr_bsdf": ([("kd", 3), ("arm", 3), ("pos", 3), ("nrm", 3), ("view_pos", 3), ("light_pos", 3)], 3, [0.08, 0]),
+    "prepare_shading_normal": ([(n, 3) for n in ("pos", "view_pos", "perturbed_nrm", "smooth_nrm", "smooth_tng", "geom_nrm")], 3, [1, 1]),
+    "shade_combine": ([("a4", 4), ("b4", 4), ("kd", 3), ("ks", 3)], 3, [1]),
+}
+
+
+def _named(name, msg):
+    return re.search(rb"(^|[^a-z_])" + name.encode() + rb"([^a-z_]|$)", msg) is not None
+
+
+@pytest.mark.parametrize("entry", ["mcs_%s_%s" % (op, way) for op in EW_OPS for way in ("fwd", "bwd")])
+def test_streaming_ops_check_every_operand_and_output(entry):
+    """Each streaming op entry refuses, before any launch, an operand with the wrong channel count, a dimension that does not
+    broadcast, a null or empty descriptor and a null output pointer, and names the operand or output.  The descriptors point
+    at fake addresses: a check that went missing would end in the failed launch of a device-less machine, whose message
+    names neither."""
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("the calls would launch on the fake pointers")
+    l = _lib.lib()
+    op, way = entry[len("mcs_"):].rsplit("_", 1)
+    operands, out_c, scalars = EW_OPS[op]
+    bwd = way == "bwd"
+    tensors = operands + [("d_out", out_c)] if bwd else operands
+    outputs = ["d_" + n for n, _ in operands] if bwd else ["out"]
+
+    def desc(C, sizes=(2, 4, 4)):
+        N, H, W = sizes
+        return _lib._desc(0x10000, (N, H, W, C), (H * W * C, W * C, C, 1))
+
+    def call(ts, outs, pbr=1):
+        sc = scalars[:-1] + [pbr] if op == "shade_combine" else scalars
+        ts = [ctypes.byref(t) if t is not None else None for t in ts]
+        args = ts[:len(operands)] + sc + ts[len(operands):] + list(outs) + [None]
+        rc = getattr(l, entry)(*args)
+        return rc, l.mcs_last_error() or b""
+
+    good = [desc(C) for _, C in tensors]
+    fake_outs = [0x20000 * (i + 1) for i in range(len(outputs))]
+    for i, (name, C) in enumerate(tensors):
+        for bad, what in ((desc(C + 1), "channels"), (desc(C, (2, 3, 4)), "broadcast")):
+            rc, msg = call(good[:i] + [bad] + good[i + 1:], fake_outs)
+            assert rc != 0 and _named(name, msg), (entry, name, what, msg)
+        for bad in (None, desc(C, (2, 0, 4))):
+            rc, msg = call(good[:i] + [bad] + good[i + 1:], fake_outs)
+            assert rc != 0 and msg == ("%s: null / empty tensor argument" % entry).encode(), (entry, name, msg)
+    for i, name in enumerate(outputs):
+        rc, msg = call(good, fake_outs[:i] + [None] + fake_outs[i + 1:])
+        assert rc != 0 and msg == ("%s: null output pointer %s" % (entry, name)).encode(), (entry, name, msg)
+    if entry == "mcs_shade_combine_bwd":
+        # 'diffuse' neither reads b4 / ks nor writes d_b4 / d_ks, so those two may be null: the call gets past every check.
+        rc, msg = call(good, [fake_outs[0], None, fake_outs[2], None], pbr=0)
+        assert rc != 0 and b"d_b4" not in msg and b"d_ks" not in msg, msg

@@ -51,6 +51,7 @@ seed_t = torch.full((1,), 7, dtype=torch.int32, device=dev)
 ou.optix_env_shade(ctx, t("mask"), t("ro"), t("pos"), nrm.detach(), t("view"), t("kd"), t("ks"), t("light"), t("pdf"), t("rows"), t("cols"), n_samples_x=N, rnd_seed=seed_t, perms=t("perms"))
 a4 = (torch.rand(2, 12, 12, 4, device=dev) + 0.5).requires_grad_(True)
 shade_combine(a4, a4 * 1.5, t("kd"), t("ks")).sum().backward()
+shade_combine(a4, a4 * 1.5, t("kd"), t("ks"), BSDF='diffuse').sum().backward()     # d_b4 / d_ks alias d_a4 / d_kd and must stay unwritten
 tex = torch.rand(64, 3, device=dev, requires_grad=True)
 texel_fetch(tex, torch.randint(0, 64, (2, 12, 12), device=dev)).sum().backward()
 # geometry gradients: rasterize backward, interpolate backward to rast (no attribute gradient), edge adjacency, antialias fwd / bwd

@@ -347,6 +347,38 @@ int mcs_texture_fwd(const mcs_texture_levels *tex, const float *uv, const float 
 int mcs_texture_bwd(const mcs_texture_levels *tex, const float *uv, const float *uv_da, int32_t B, int32_t H, int32_t W, int32_t filter_mode,
                     int32_t boundary_mode, const float *d_out, float *const *d_tex, float *d_uv, float *d_uv_da, mcs_stream stream);
 
+/* ---- DMTet geometry: marching_tets and sdf_reg_loss (geometry/dmtet.py:91-153); semantics in csrc/dmtet.cu.  All arrays are device
+ *      memory.  Static tables of one tet grid (V vertices, T tets, E unique edges), built once by the caller:
+ *        edges [E,2] int32, 8-byte aligned: the unique vertex pairs of the tets' six base edges, each as (min, max), sorted
+ *          lexicographically;
+ *        tets [T,4] int32, 16-byte aligned; tet_edges [T,6] int32: the row of `edges` of the tet's base edges (0,1) (0,2) (0,3) (1,2)
+ *          (1,3) (2,3);
+ *        v2e_offsets [V+1] / v2e_edges int32: for vertex v, v2e_edges[v2e_offsets[v] .. v2e_offsets[v+1]) lists the rows of `edges` with
+ *          v as an end, in ascending order (a row whose two ends are v is listed twice).
+ *      sdf [V] and pos [V,3] are fp32 with the given element strides.
+ *      mcs_dmtet_count writes vid [E] (the output vertex of each edge, -1 where it does not cross), tet_prefix [T,2] (exclusive prefixes
+ *      of the 1- and 2-triangle tets, 8-byte aligned) and counts [3] = (vertices M, 1-triangle tets n1, 2-triangle tets n2); workspace:
+ *      mcs_dmtet_workspace_bytes(E, T) bytes, 8-byte aligned, contents ignored on entry.  mcs_dmtet_emit then writes verts [M,3] fp32,
+ *      faces [n1 + 2 n2, 3] int64 and uv_idx [n1 + 2 n2, 3] int64; the caller sizes them from counts read back after the count phase.
+ *      mcs_dmtet_bwd overwrites d_pos [V,3] and d_sdf [V] (contiguous) from d_verts [M,3] (contiguous) by a per-vertex gather, no atomics.
+ *      mcs_sdf_reg_fwd: loss (one float) = the reference's sdf_reg_loss over the edge list edges [E,2] (any vertex pairs), m (one float) =
+ *      the number of masked edges; partials: mcs_sdf_reg_num_partials(E) x 3 doubles of scratch.  mcs_sdf_reg_bwd overwrites d_sdf [V] from
+ *      the upstream gradient d_loss (one float on the device), with v2e_* the CSR of that edge list.  No entry synchronises the host. */
+#define MCS_DMTET_TILE 2048
+int64_t mcs_dmtet_workspace_bytes(int32_t E, int32_t T);
+int mcs_dmtet_count(const float *sdf, int64_t sdf_stride, const int32_t *edges, int32_t E, const int32_t *tets, int32_t T, int32_t *vid,
+                    int32_t *tet_prefix, int32_t *counts, void *workspace, mcs_stream stream);
+int mcs_dmtet_emit(const float *pos, int64_t pos_stride0, int64_t pos_stride1, const float *sdf, int64_t sdf_stride, const int32_t *edges, int32_t E,
+                   const int32_t *tets, const int32_t *tet_edges, int32_t T, const int32_t *vid, const int32_t *tet_prefix, const int32_t *counts,
+                   float *verts, int64_t *faces, int64_t *uv_idx, mcs_stream stream);
+int mcs_dmtet_bwd(const float *pos, int64_t pos_stride0, int64_t pos_stride1, const float *sdf, int64_t sdf_stride, int32_t V, const int32_t *edges,
+                  int32_t E, const int32_t *vid, const int32_t *v2e_offsets, const int32_t *v2e_edges, const float *d_verts, float *d_pos, float *d_sdf,
+                  mcs_stream stream);
+int32_t mcs_sdf_reg_num_partials(int32_t E);
+int mcs_sdf_reg_fwd(const float *sdf, int64_t sdf_stride, const int32_t *edges, int32_t E, double *partials, float *loss, float *m, mcs_stream stream);
+int mcs_sdf_reg_bwd(const float *sdf, int64_t sdf_stride, int32_t V, const int32_t *edges, const int32_t *v2e_offsets, const int32_t *v2e_edges,
+                    const float *m, const float *d_loss, float *d_sdf, mcs_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

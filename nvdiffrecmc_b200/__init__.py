@@ -7,6 +7,7 @@ Sub-packages mirror the reference layout:
     nvdiffrecmc_b200.renderutils  <->  render/renderutils  (pbr_bsdf, prepare_shading_normal, ... )
     nvdiffrecmc_b200.denoiser     <->  denoiser/denoiser.py (BilateralDenoiser)
     nvdiffrecmc_b200.light        <->  render/light.py      (EnvironmentLight)
+    nvdiffrecmc_b200.dmtet        <->  geometry/dmtet.py    (marching_tets, sdf_reg_loss)
 All of them call hand-written CUDA kernels in lib/libmcshade.so through the C ABI in include/mcshade.h.
 """
 from . import _lib  # noqa: F401

@@ -15,7 +15,7 @@ _CSRC = os.path.join(_PKG, "csrc")
 _LIBDIR = os.path.join(_PKG, "lib")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
 SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu",
-           "mlptexture.cu"]
+           "mlptexture.cu", "dmtet.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
@@ -148,6 +148,13 @@ _SIGS = {
     "mcs_mlptex_bwd": ([_P, C.c_int64] + [_P] * 4 + [C.c_int32, C.c_int32] + [_P] * 8, C.c_int),
     "mcs_texture_fwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P, _P], C.c_int),
     "mcs_texture_bwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P] * 5, C.c_int),
+    "mcs_dmtet_workspace_bytes": ([C.c_int32, C.c_int32], C.c_int64),
+    "mcs_dmtet_count": ([_P, C.c_int64, _P, C.c_int32, _P, C.c_int32] + [_P] * 5, C.c_int),
+    "mcs_dmtet_emit": ([_P, C.c_int64, C.c_int64, _P, C.c_int64, _P, C.c_int32, _P, _P, C.c_int32] + [_P] * 7, C.c_int),
+    "mcs_dmtet_bwd": ([_P, C.c_int64, C.c_int64, _P, C.c_int64, C.c_int32, _P, C.c_int32] + [_P] * 7, C.c_int),
+    "mcs_sdf_reg_num_partials": ([C.c_int32], C.c_int32),
+    "mcs_sdf_reg_fwd": ([_P, C.c_int64, _P, C.c_int32] + [_P] * 4, C.c_int),
+    "mcs_sdf_reg_bwd": ([_P, C.c_int64, C.c_int32] + [_P] * 7, C.c_int),
 }
 EXPORTED_SYMBOLS = sorted(_SIGS)
 
@@ -178,7 +185,7 @@ def lib():
 LAUNCHES = collections.Counter()
 _KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "rasterize_peel": 2,
                      "antialias_topology": 2, "hashgrid_bwd_both": 2, "mlptex_bwd_dw": 2,
-                     "texture_fwd": 1, "texture_bwd": 1}
+                     "texture_fwd": 1, "texture_bwd": 1, "dmtet_count": 1, "dmtet_emit": 1, "dmtet_bwd": 1, "sdf_reg_fwd": 2, "sdf_reg_bwd": 1}
 
 
 def check(status, what):

@@ -1,4 +1,4 @@
-"""ctypes binding of libmcshade.so (C ABI declared in include/mcshade.h) + the in-tree build recipe.
+"""ctypes binding of libmcshade.so, read from the C ABI's header include/mcshade.h, + the in-tree build recipe.
 
 The product path has NO fallback: if the shared library is missing or a call fails, a RuntimeError
 is raised (the reference silently drops CUDA/OptiX errors, optixutils/c_src/common.h:37-61).
@@ -6,6 +6,7 @@ is raised (the reference silently drops CUDA/OptiX errors, optixutils/c_src/comm
 import collections
 import ctypes as C
 import os
+import re
 import subprocess
 import sys
 from concurrent.futures import ThreadPoolExecutor
@@ -13,6 +14,7 @@ from concurrent.futures import ThreadPoolExecutor
 _PKG = os.path.dirname(os.path.abspath(__file__))
 _CSRC = os.path.join(_PKG, "csrc")
 _LIBDIR = os.path.join(_PKG, "lib")
+HEADER = os.path.join(os.path.dirname(_PKG), "include", "mcshade.h")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
 SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu",
            "mlptexture.cu", "dmtet.cu"]
@@ -32,7 +34,7 @@ def build(force=False, verbose=False):
     objdir = os.path.join(_LIBDIR, "obj")
     os.makedirs(objdir, exist_ok=True)
     hdrs = [os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h"))]
-    hdrs.append(os.path.join(os.path.dirname(_PKG), "include", "mcshade.h"))
+    hdrs.append(HEADER)
     newest_hdr = max(os.path.getmtime(h) for h in hdrs)
     nvcc = _nvcc()
 
@@ -62,101 +64,52 @@ def build(force=False, verbose=False):
     return LIB_PATH
 
 
-class mcs_hashgrid_levels(C.Structure):
-    _fields_ = [("n_levels", C.c_int32), ("offset", C.c_uint32 * 17), ("res", C.c_uint32 * 16), ("scale", C.c_float * 16), ("dense_mask", C.c_uint32)]
+# The binding is read from include/mcshade.h, the one place the ABI is written down: its structs become ctypes Structures and every
+# mcs_* prototype gets declared argument and result types.  The type map is closed, so a header edit it does not cover fails at import.
+_SCALARS = {"int": C.c_int, "int32_t": C.c_int32, "uint32_t": C.c_uint32, "int64_t": C.c_int64, "float": C.c_float, "mcs_stream": C.c_void_p}
 
 
-class mcs_texture_levels(C.Structure):
-    _fields_ = [("n_levels", C.c_int32), ("C", C.c_int32), ("ptr", C.c_void_p * 16), ("h", C.c_int32 * 16), ("w", C.c_int32 * 16),
-                ("batch_stride", C.c_int64 * 16)]
+def _ctype(decl, where, result=False):
+    """ctypes type of the C type `decl` (written without a name, e.g. 'const mcs_tensor *') in the declaration `where`."""
+    t = " ".join(decl.replace("*", " * ").split())
+    if result and t == "const char *":
+        return C.c_char_p
+    if t == "const mcs_tensor *":
+        return C.POINTER(mcs_tensor)
+    if "*" in t:
+        return C.c_void_p
+    if t not in _SCALARS:
+        raise TypeError("include/mcshade.h: %s: no ctypes type for the C type '%s'" % (where, t))
+    return _SCALARS[t]
 
 
-class mcs_tensor(C.Structure):
-    _fields_ = [("ptr", C.c_void_p), ("sizes", C.c_int32 * 4), ("strides", C.c_int32 * 4)]
+def _structs(src):
+    """{name: Structure} of every `typedef struct mcs_X { ... } mcs_X;` in the comment-free header text `src`."""
+    out = {}
+    for name, body in re.findall(r"typedef struct (mcs_\w+)\s*\{([^}]*)\}\s*\1\s*;", src):
+        fields = [(f, _ctype(decl, name) * int(n) if n else _ctype(decl, name))
+                  for decl, f, n in re.findall(r"([^;]*?)\b(\w+)\s*(?:\[(\d+)\])?\s*;", body)]
+        out[name] = type(name, (C.Structure,), {"_fields_": fields})
+    return out
 
 
+def _prototypes(src):
+    """{name: ([argument types], result type)} of every mcs_* prototype in the comment-free header text `src`."""
+    sigs = {}
+    for res, name, params in re.findall(r"^([A-Za-z_][\w \*]*?)\b(mcs_\w+)\s*\(([^)]*)\)\s*;", src, re.M):
+        args = [] if params.strip() == "void" else [_ctype(re.sub(r"\w+\s*$", "", p), name) for p in params.split(",")]
+        sigs[name] = (args, _ctype(res, name, result=True))
+    return sigs
+
+
+with open(HEADER) as _f:
+    _src = re.sub(r"/\*.*?\*/", " ", _f.read(), flags=re.S)
+_STRUCTS = _structs(_src)
+mcs_tensor, mcs_hashgrid_levels, mcs_texture_levels = _STRUCTS["mcs_tensor"], _STRUCTS["mcs_hashgrid_levels"], _STRUCTS["mcs_texture_levels"]
+_ABI_VERSION = int(re.search(r"#define MCS_ABI_VERSION (\d+)", _src).group(1))
+_SIGNATURES = _prototypes(_src)
+EXPORTED_SYMBOLS = sorted(_SIGNATURES)
 _lib = None
-_T = C.POINTER(mcs_tensor)
-_P = C.c_void_p
-_SIGS = {
-    "mcs_abi_version": ([], C.c_int),
-    "mcs_last_error": ([], C.c_char_p),
-    "mcs_ctx_create": ([C.POINTER(_P)], C.c_int),
-    "mcs_ctx_destroy": ([_P], C.c_int),
-    "mcs_bvh_build": ([_P, _P, C.c_int32, _P, C.c_int32, C.c_uint32, _P], C.c_int),
-    "mcs_bvh_export": ([_P] * 8, C.c_int),
-    "mcs_bvh_export_shadow": ([_P] * 5, C.c_int),
-    "mcs_trace_visibility": ([_P, _P, _P, C.c_int64, _P, _P], C.c_int),
-    "mcs_trace_closest": ([_P, _P, _P, C.c_int64, _P, _P, _P], C.c_int),
-    "mcs_trace_closest_after": ([_P, _P, _P, _P, C.c_int64, _P, _P, _P], C.c_int),
-    "mcs_env_shade_fwd": ([_P] + [_T] * 12 + [C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_float, C.c_int32, _P, _P, _P, _P, _P, C.c_int32, _P], C.c_int),
-    "mcs_env_shade_bwd_replay": ([_T] * 6 + [C.c_uint32, C.c_uint32, C.c_float, _T, _T, _P, _P, C.c_int32] + [_P] * 6, C.c_int),
-    "mcs_env_shade_records": ([_P] + [_T] * 12 + [C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_float, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
-    "mcs_env_shade_bwd": ([_P] + [_T] * 12 + [C.c_uint32, C.c_uint32, C.c_uint32, _P, C.c_float, C.c_int32, _T, _T] + [_P] * 7, C.c_int),
-    "mcs_bilateral_fwd": ([_T, _T, _T, C.c_float, _P, _P], C.c_int),
-    "mcs_bilateral_bwd": ([_T, _T, C.c_float, _T, _P, _P], C.c_int),
-    "mcs_bilateral_fwd2": ([_T, _T, _T, _T, C.c_float, _P, _P, _P], C.c_int),
-    "mcs_bilateral_bwd2": ([_T, _T, C.c_float, _T, _T, _P, _P, _P], C.c_int),
-    "mcs_lambert_fwd": ([_T] * 2 + [_P] * 2, C.c_int),
-    "mcs_lambert_bwd": ([_T] * 3 + [_P] * 3, C.c_int),
-    "mcs_frostbite_fwd": ([_T] * 4 + [_P] * 2, C.c_int),
-    "mcs_frostbite_bwd": ([_T] * 5 + [_P] * 5, C.c_int),
-    "mcs_fresnel_shlick_fwd": ([_T] * 3 + [_P] * 2, C.c_int),
-    "mcs_fresnel_shlick_bwd": ([_T] * 4 + [_P] * 4, C.c_int),
-    "mcs_ndf_ggx_fwd": ([_T] * 2 + [_P] * 2, C.c_int),
-    "mcs_ndf_ggx_bwd": ([_T] * 3 + [_P] * 3, C.c_int),
-    "mcs_lambda_ggx_fwd": ([_T] * 2 + [_P] * 2, C.c_int),
-    "mcs_lambda_ggx_bwd": ([_T] * 3 + [_P] * 3, C.c_int),
-    "mcs_masking_smith_fwd": ([_T] * 3 + [_P] * 2, C.c_int),
-    "mcs_masking_smith_bwd": ([_T] * 4 + [_P] * 4, C.c_int),
-    "mcs_pbr_specular_fwd": ([_T] * 5 + [C.c_float, _P, _P], C.c_int),
-    "mcs_pbr_specular_bwd": ([_T] * 5 + [C.c_float, _T] + [_P] * 6, C.c_int),
-    "mcs_pbr_bsdf_fwd": ([_T] * 6 + [C.c_float, C.c_int32, _P, _P], C.c_int),
-    "mcs_pbr_bsdf_bwd": ([_T] * 6 + [C.c_float, C.c_int32, _T] + [_P] * 7, C.c_int),
-    "mcs_prepare_shading_normal_fwd": ([_T] * 6 + [C.c_int32, C.c_int32, _P, _P], C.c_int),
-    "mcs_prepare_shading_normal_bwd": ([_T] * 6 + [C.c_int32, C.c_int32, _T] + [_P] * 7, C.c_int),
-    "mcs_image_loss_num_partials": ([C.c_int32] * 3, C.c_int),
-    "mcs_image_loss_fwd": ([_T, _T, C.c_int32, C.c_int32, _P, _P], C.c_int),
-    "mcs_image_loss_bwd": ([_T, _T, C.c_int32, C.c_int32, _T, _P, _P, _P], C.c_int),
-    "mcs_xfm_fwd": ([_T, _T, C.c_int32, _P, _P], C.c_int),
-    "mcs_xfm_bwd": ([_T, _T, _T, C.c_int32, _P, _P], C.c_int),
-    "mcs_update_pdf": ([_T, _P, _P, _P, _P, _P], C.c_int),
-    "mcs_shade_combine_fwd": ([_T, _T, _T, _T, C.c_int32, _P, _P], C.c_int),
-    "mcs_shade_combine_bwd": ([_T, _T, _T, _T, C.c_int32, _T, _P, _P, _P, _P, _P], C.c_int),
-    "mcs_texel_fetch_fwd": ([_P, C.c_int64, C.c_int32, _P, C.c_int64, _P, _P], C.c_int),
-    "mcs_texel_fetch_bwd": ([C.c_int64, C.c_int32, _P, C.c_int64, _P, _P, _P], C.c_int),
-    "mcs_rasterize": ([_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
-    "mcs_rasterize_peel": ([_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
-    "mcs_interpolate_fwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
-    "mcs_interpolate_bwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
-    "mcs_interpolate_bwd_rast": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P], C.c_int),
-    "mcs_rasterize_bwd": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P], C.c_int),
-    "mcs_rast_db": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P], C.c_int),
-    "mcs_rasterize_bwd_db": ([_P, C.c_int64, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P], C.c_int),
-    "mcs_interpolate_da_fwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P],
-                               C.c_int),
-    "mcs_interpolate_da_bwd": ([_P, C.c_int64, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
-                                _P, _P], C.c_int),
-    "mcs_aa_topology_workspace_bytes": ([C.c_int32], C.c_int64),
-    "mcs_aa_topology": ([_P, C.c_int32, _P, _P, _P], C.c_int),
-    "mcs_antialias_fwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P], C.c_int),
-    "mcs_antialias_bwd": ([_P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P], C.c_int),
-    "mcs_hashgrid_fwd": ([_P, C.c_int64, _P, _P, _P, _P], C.c_int),
-    "mcs_hashgrid_bwd": ([_P, C.c_int64, _P, _P, _P, _P, _P, _P], C.c_int),
-    "mcs_mlptex_workspace_bytes": ([C.c_int64, C.c_int32, C.c_int32], C.c_int64),
-    "mcs_mlptex_fwd": ([_P, C.c_int64] + [_P] * 4 + [C.c_int32, C.c_int32] + [_P] * 4, C.c_int),
-    "mcs_mlptex_bwd": ([_P, C.c_int64] + [_P] * 4 + [C.c_int32, C.c_int32] + [_P] * 8, C.c_int),
-    "mcs_texture_fwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P, _P], C.c_int),
-    "mcs_texture_bwd": ([_P, _P, _P] + [C.c_int32] * 5 + [_P] * 5, C.c_int),
-    "mcs_dmtet_workspace_bytes": ([C.c_int32, C.c_int32], C.c_int64),
-    "mcs_dmtet_count": ([_P, C.c_int64, _P, C.c_int32, _P, C.c_int32] + [_P] * 5, C.c_int),
-    "mcs_dmtet_emit": ([_P, C.c_int64, C.c_int64, _P, C.c_int64, _P, C.c_int32, _P, _P, C.c_int32] + [_P] * 7, C.c_int),
-    "mcs_dmtet_bwd": ([_P, C.c_int64, C.c_int64, _P, C.c_int64, C.c_int32, _P, C.c_int32] + [_P] * 7, C.c_int),
-    "mcs_sdf_reg_num_partials": ([C.c_int32], C.c_int32),
-    "mcs_sdf_reg_fwd": ([_P, C.c_int64, _P, C.c_int32] + [_P] * 4, C.c_int),
-    "mcs_sdf_reg_bwd": ([_P, C.c_int64, C.c_int32] + [_P] * 7, C.c_int),
-}
-EXPORTED_SYMBOLS = sorted(_SIGS)
 
 
 def lib():
@@ -169,12 +122,12 @@ def lib():
             "libmcshade.so not found at %s -- build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(nvcc, sm_90a). There is no CPU / PyTorch fallback for the hot path." % LIB_PATH)
     l = C.CDLL(LIB_PATH)
-    for name, (args, res) in _SIGS.items():
+    for name, (args, res) in _SIGNATURES.items():
         fn = getattr(l, name)          # AttributeError if the symbol is missing
         fn.argtypes = args
         fn.restype = res
-    if l.mcs_abi_version() != 2:
-        raise RuntimeError("libmcshade ABI version mismatch")
+    if l.mcs_abi_version() != _ABI_VERSION:
+        raise RuntimeError("libmcshade ABI version mismatch: the library has %d, include/mcshade.h %d" % (l.mcs_abi_version(), _ABI_VERSION))
     _lib = l
     return l
 

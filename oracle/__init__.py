@@ -1,9 +1,9 @@
 """CPU oracle for the nvdiffrecmc hot path -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-numpy/ctypes wrappers around the four C restatements in this directory (see each file's header for what it restates and how it is
-pinned): ``Oracle`` and ``Scene`` here wrap ``mcoracle.c``; ``oracle.geometry``, ``oracle.hashgrid`` and ``oracle.texture`` wrap the C file
-of the same name.  Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import
-this package; ``nvdiffrecmc_b200`` never does.
+numpy/ctypes wrappers around the six C restatements in this directory (see each file's header for what it restates and how it is
+pinned): ``Oracle`` and ``Scene`` here wrap ``mcoracle.c``; ``oracle.geometry``, ``oracle.hashgrid``, ``oracle.texture``,
+``oracle.mlptexture`` and ``oracle.dmtet`` wrap the C file of the same name.  Only ``tests/``, ``__graft_entry__.smoke()`` and
+``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import this package; ``nvdiffrecmc_b200`` never does.
 
 ``build()`` compiles every library twice from the same source: fp32 (the oracle proper, compared with the CUDA kernels) and fp64
 (``f64=True``), used only to validate derivatives and hand-derived adjoints by finite differences.  ``CLib`` is the wrappers' common base:
@@ -22,7 +22,9 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _BUILD = os.path.join(_HERE, "_build")
-LIBS = {"mcoracle": ["mcoracle.c", "detmath.h"], "geometry": ["geometry.c"], "hashgrid": ["hashgrid.c"], "texture": ["texture.c"]}  # source, headers
+# library: [its source, then the files that source #includes]
+LIBS = {"mcoracle": ["mcoracle.c", "detmath.h"], "geometry": ["geometry.c"], "hashgrid": ["hashgrid.c"], "texture": ["texture.c"],
+        "mlptexture": ["mlptexture.c", "hashgrid.c"], "dmtet": ["dmtet.c"]}
 
 
 def _cpu_has_fma():

@@ -2,26 +2,13 @@
 
 numpy/ctypes wrapper around ``oracle/dmtet.c`` (the contract is stated in nvdiffrecmc_b200/csrc/dmtet.cu).  Two builds of the same source:
 fp32 (``dmtet_oracle()``, compared bit for bit with the CUDA vertices, faces, uv_idx, d pos and d sdf) and fp64 (``dmtet_oracle(f64=True)``,
-checked by finite differences).  ``build()`` compiles both; ``__graft_entry__.build()`` calls it.
+checked by finite differences).  ``oracle.build()`` compiles both from ``oracle.LIBS``.
 """
 import ctypes as C
-import os
 
 import numpy as np
 
-from oracle import _CFLAGS, _HERE, _I, _I64, _P, REAL, CLib, _compile, _lib_path
-
-SOURCE = os.path.join(_HERE, "dmtet.c")
-
-
-def _build(f64, force=False):
-    _compile(["gcc"] + _CFLAGS + (["-DORACLE_F64"] if f64 else []) + [SOURCE, "-lm"], _lib_path("dmtet", f64), [SOURCE], force)
-
-
-def build(force=False):
-    """Compile oracle/dmtet.c with gcc, fp32 and fp64 (-DORACLE_F64), into oracle/_build/."""
-    for f64 in (False, True):
-        _build(f64, force)
+from oracle import _I, _I64, _P, REAL, CLib
 
 
 class DmtetOracle(CLib):
@@ -37,18 +24,6 @@ class DmtetOracle(CLib):
         "dmt_reg_fwd": ([_I64, _P, _P, _P], C.c_double),
         "dmt_reg_bwd": ([_I64, _I64, _P, _P, REAL, _P], None),
     }
-
-    def __init__(self, f64=False):
-        # CLib.__init__ builds from oracle.LIBS; this library has its own recipe (build() above), the loading is the same
-        self.f64 = f64
-        self.dt, self.real = (np.float64, C.c_double) if f64 else (np.float32, C.c_float)
-        _build(f64)
-        self.lib = C.CDLL(_lib_path(self.LIB, f64))
-        for name, (args, res) in self.SIGS.items():
-            fn = getattr(self.lib, name)          # AttributeError if the library does not export it
-            fn.argtypes = [self.real if a is REAL else a for a in args]
-            fn.restype = res
-        assert self.lib.dmt_sizeof_real() == C.sizeof(self.real)
 
     def tables(self, tet, V):
         """Static tables of a grid: dict(edges [E,2], tet_edges [T,6], v2e_offsets [V+1], v2e_edges [2E]), int32."""

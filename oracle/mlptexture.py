@@ -4,28 +4,18 @@ numpy/ctypes wrapper around ``oracle/mlptexture.c`` (the contract is stated in n
 ``oracle/hashgrid.c`` for the encoding, so the library also exports the hash-grid oracle's functions and ``MlpTextureOracle`` is a
 ``HashGridOracle`` (``levels``, ``forward``, ``backward``) with the MLP texture added.  Two builds of the same source: fp32
 (``mlptexture_oracle()``, compared bit for bit with the CUDA output, saved encoding, d texc and d W) and fp64 (``mlptexture_oracle(f64=True)``,
-checked by finite differences).  ``build()`` compiles both; ``__graft_entry__.build()`` calls it.
+checked by finite differences).  ``oracle.build()`` compiles both from ``oracle.LIBS``.
 """
 import ctypes as C
 import os
 
 import numpy as np
 
-from oracle import _CFLAGS, _HERE, _I, _I64, _P, REAL, _compile, _lib_path
+from oracle import _HERE, _I, _I64, _P, LIBS
 from oracle.hashgrid import HashGridOracle
 
-SOURCES = [os.path.join(_HERE, "mlptexture.c"), os.path.join(_HERE, "hashgrid.c")]     # source, included file
+SOURCES = [os.path.join(_HERE, s) for s in LIBS["mlptexture"]]      # paths of the library's source and the hashgrid.c it includes
 MLPTEX_CHUNK = 1024          # MCS_MLPTEX_CHUNK: points per d W chunk partial
-
-
-def _build(f64, force=False):
-    _compile(["gcc"] + _CFLAGS + (["-DORACLE_F64"] if f64 else []) + [SOURCES[0], "-lm"], _lib_path("mlptexture", f64), SOURCES, force)
-
-
-def build(force=False):
-    """Compile oracle/mlptexture.c with gcc, fp32 and fp64 (-DORACLE_F64), into oracle/_build/."""
-    for f64 in (False, True):
-        _build(f64, force)
 
 
 class MlpTextureOracle(HashGridOracle):
@@ -35,18 +25,6 @@ class MlpTextureOracle(HashGridOracle):
         "mlt_fwd": ([_P, _I64] + [_P] * 3 + [_I, _P, _P, _P, C.c_uint32, _I, _I] + [_P] * 3, None),
         "mlt_bwd": ([_P, _I64] + [_P] * 3 + [_I, _P, _P, _P, C.c_uint32, _I, _I] + [_P] * 5, None),
     })
-
-    def __init__(self, f64=False):
-        # CLib.__init__ builds from oracle.LIBS; this library has its own recipe (build() above), the loading is the same
-        self.f64 = f64
-        self.dt, self.real = (np.float64, C.c_double) if f64 else (np.float32, C.c_float)
-        _build(f64)
-        self.lib = C.CDLL(_lib_path(self.LIB, f64))
-        for name, (args, res) in self.SIGS.items():
-            fn = getattr(self.lib, name)          # AttributeError if the library does not export it
-            fn.argtypes = [self.real if a is REAL else a for a in args]
-            fn.restype = res
-        assert self.lib.hg_sizeof_real() == C.sizeof(self.real)
 
     def exp(self, x):
         """The MLP texture's exp (csrc/mlptexture.cu, fp32 build; libm exp in the fp64 build)."""

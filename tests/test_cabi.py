@@ -1,7 +1,10 @@
-"""CPU: the C-ABI shared library loads and exports every symbol include/mcshade.h declares (no compute without a GPU)."""
+"""CPU: the C-ABI shared library loads and exports every symbol include/mcshade.h declares, and the binding read from the header
+agrees with it (no compute without a GPU)."""
 import ctypes
 import os
 import re
+import subprocess
+import tempfile
 
 import pytest
 
@@ -11,9 +14,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 def _declared():
+    """{name: parameter count} of every prototype of the header."""
     src = open(os.path.join(ROOT, "include", "mcshade.h")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(mcs_[a-z0-9_]+)\s*\(", src)))
+    return {n: 0 if p.strip() == "void" else p.count(",") + 1 for n, p in re.findall(r"\b(mcs_[a-z0-9_]+)\s*\(([^)]*)\)", src)}
 
 
 def test_library_is_built_in_tree_and_loads():
@@ -24,17 +28,66 @@ def test_library_is_built_in_tree_and_loads():
 
 
 def test_every_declared_symbol_is_exported_and_bound():
-    names = _declared()
-    assert len(names) >= 30
+    declared = _declared()
+    assert len(declared) >= 30
     raw = ctypes.CDLL(_lib.LIB_PATH)
-    for n in names:
+    for n in declared:
         assert hasattr(raw, n), "missing export: " + n
-    assert sorted(_lib.EXPORTED_SYMBOLS) == names, "Python binding table and header disagree"
+    assert _lib.EXPORTED_SYMBOLS == sorted(declared)
+    l = _lib.lib()
+    for n, n_params in declared.items():
+        fn = getattr(l, n)
+        assert fn.argtypes is not None, "not bound: " + n
+        assert len(fn.argtypes) == n_params, n
+
+
+_T, _P = ctypes.POINTER(_lib.mcs_tensor), ctypes.c_void_p
+PINNED = {
+    "mcs_env_shade_fwd": ([_P] + [_T] * 12 + [ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint32, _P, ctypes.c_float, ctypes.c_int32, _P, _P, _P, _P, _P,
+                                             ctypes.c_int32, _P], ctypes.c_int),
+    "mcs_dmtet_emit": ([_P, ctypes.c_int64, ctypes.c_int64, _P, ctypes.c_int64, _P, ctypes.c_int32, _P, _P, ctypes.c_int32] + [_P] * 7, ctypes.c_int),
+    "mcs_texture_bwd": ([_P, _P, _P] + [ctypes.c_int32] * 5 + [_P] * 5, ctypes.c_int),
+    "mcs_mlptex_bwd": ([_P, ctypes.c_int64] + [_P] * 4 + [ctypes.c_int32, ctypes.c_int32] + [_P] * 8, ctypes.c_int),
+    "mcs_last_error": ([], ctypes.c_char_p),
+    "mcs_aa_topology_workspace_bytes": ([ctypes.c_int32], ctypes.c_int64),
+}
+
+
+@pytest.mark.parametrize("name", sorted(PINNED))
+def test_pinned_signatures(name):
+    args, res = PINNED[name]
+    fn = getattr(_lib.lib(), name)
+    assert list(fn.argtypes) == args and fn.restype is res
+
+
+def test_struct_layout_matches_the_c_compiler():
+    """Each header struct's ctypes layout equals gcc's: its size, and every field's offset and size."""
+    structs = [_lib.mcs_tensor, _lib.mcs_hashgrid_levels, _lib.mcs_texture_levels]
+    prints, want = [], []
+    for s in structs:
+        n = s.__name__
+        prints.append('printf("%s %%zu\\n", sizeof(%s));' % (n, n))
+        want.append("%s %d" % (n, ctypes.sizeof(s)))
+        for f, _ in s._fields_:
+            prints.append('printf("%s.%s %%zu %%zu\\n", offsetof(%s, %s), sizeof(((%s *)0)->%s));' % (n, f, n, f, n, f))
+            want.append("%s.%s %d %d" % (n, f, getattr(s, f).offset, getattr(s, f).size))
+    with tempfile.TemporaryDirectory() as d:
+        c, exe = os.path.join(d, "layout.c"), os.path.join(d, "layout")
+        open(c, "w").write('#include <stddef.h>\n#include <stdio.h>\n#include "mcshade.h"\nint main(void){\n%s\nreturn 0; }\n' % "\n".join(prints))
+        subprocess.run(["gcc", "-std=c99", "-Wall", "-Werror", "-I", os.path.join(ROOT, "include"), c, "-o", exe], check=True)
+        got = subprocess.run([exe], check=True, capture_output=True, text=True).stdout.split("\n")[:-1]
+    assert got == want
+
+
+@pytest.mark.parametrize("src,where", [("int mcs_x(size_t n);", "mcs_x"), ("size_t mcs_y(int n);", "mcs_y"),
+                                       ("typedef struct mcs_z { size_t n; } mcs_z;", "mcs_z")])
+def test_unknown_c_type_is_an_error_naming_the_declaration(src, where):
+    parse = _lib._structs if src.startswith("typedef") else _lib._prototypes
+    with pytest.raises(TypeError, match=r"\b%s\b.*'size_t'" % where):
+        parse(src)
 
 
 def test_header_is_plain_c():
-    import subprocess
-    import tempfile
     with tempfile.TemporaryDirectory() as d:
         c = os.path.join(d, "t.c")
         open(c, "w").write('#include "mcshade.h"\nint main(void){ mcs_tensor t; (void)t; return MCS_ABI_VERSION == 2 ? 0 : 1; }\n')

@@ -7,18 +7,25 @@ import re
 import pytest
 
 from oracle import LIBS, REAL, Oracle
+from oracle.dmtet import DmtetOracle
 from oracle.geometry import GeometryOracle
 from oracle.hashgrid import HashGridOracle
+from oracle.mlptexture import MlpTextureOracle
 from oracle.texture import TextureOracle
 
 ORACLE_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
-WRAPPERS = [(Oracle, 47), (GeometryOracle, 14), (HashGridOracle, 4), (TextureOracle, 4)]     # exports of each library at the time of writing
+WRAPPERS = [(Oracle, 47), (GeometryOracle, 14), (HashGridOracle, 4), (TextureOracle, 4), (MlpTextureOracle, 7),
+            (DmtetOracle, 9)]     # exports of each library at the time of writing
 
 
-def _exports(source):
-    """Names of the non-static orc_* / geo_* / hg_* / tex_* function definitions of a C file."""
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ORACLE_DIR, source)).read(), flags=re.S)
-    return sorted(re.findall(r"^(?!static\b)[A-Za-z_][\w \*]*?\b((?:orc|geo|hg|tex)_\w+)\s*\([^;{]*\)\s*\{", src, re.M))
+def _exports(lib):
+    """Names of the non-static orc_* / geo_* / hg_* / tex_* / mlt_* / dmt_* function definitions of every C file of a library."""
+    names = []
+    for source in LIBS[lib]:
+        if source.endswith(".c"):
+            src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ORACLE_DIR, source)).read(), flags=re.S)
+            names += re.findall(r"^(?!static\b)[A-Za-z_][\w \*]*?\b((?:orc|geo|hg|tex|mlt|dmt)_\w+)\s*\([^;{]*\)\s*\{", src, re.M)
+    return sorted(names)
 
 
 def test_every_library_has_a_wrapper():
@@ -27,7 +34,7 @@ def test_every_library_has_a_wrapper():
 
 @pytest.mark.parametrize("cls,n", WRAPPERS, ids=[cls.LIB for cls, _ in WRAPPERS])
 def test_signature_table_names_exactly_the_exports(cls, n):
-    names = _exports(LIBS[cls.LIB][0])
+    names = _exports(cls.LIB)
     assert len(names) >= n, "the definition pattern no longer finds the exports"
     assert sorted(cls.SIGS) == names, "signature table and source disagree"
 

@@ -292,7 +292,7 @@ def _envshade_struct(real):
             ("pos_grad", C.c_void_p), ("nrm_grad", C.c_void_p), ("kd_grad", C.c_void_p), ("ks_grad", C.c_void_p),
             ("light_grad", C.c_void_p),
             ("rec_texel", C.c_void_p), ("rec_vis", C.c_void_p), ("counters", C.c_void_p),
-            ("s_pos", C.c_void_p), ("s_nrm", C.c_void_p), ("s_kd", C.c_void_p), ("s_ks", C.c_void_p),
+            ("s_pos", C.c_void_p), ("s_nrm", C.c_void_p), ("s_kd", C.c_void_p), ("s_ks", C.c_void_p), ("abs_terms", C.c_int32),
         ]
     return S
 
@@ -571,10 +571,11 @@ class Oracle(CLib):
     # ------------------------------------------------------------------ env shade
     def env_shade(self, scene, mask, ro, gb_pos, gb_normal, gb_view_pos, gb_kd, gb_ks, light, pdf, rows, cols, perms,
                   BSDF="pbr", n_samples_x=8, rnd_seed=0, shadow_scale=1.0, batch_offset=0, vis_mode="brute",
-                  grads=None, records=False, counters=False, parallel_bwd=False, sampling_gbuffer=None):
+                  grads=None, records=False, counters=False, parallel_bwd=False, sampling_gbuffer=None, abs_terms=False):
         """Forward (grads=None) -> (diff, spec[, records][, counters]);
         backward (grads=(diff_grad, spec_grad)) -> (pos_grad, nrm_grad, kd_grad, ks_grad, light_grad).
-        Mirrors env_shade_fwd / env_shade_bwd, render/optixutils/c_src/torch_bindings.cpp:123-272."""
+        Mirrors env_shade_fwd / env_shade_bwd, render/optixutils/c_src/torch_bindings.cpp:123-272.
+        abs_terms (test-only): every output is the sum of the absolute values of its per-ray terms instead (see OrcEnvShade)."""
         assert scene is None or scene.orc is self, "scene was built by a different Oracle instance (fp32 vs fp64 layouts differ)"
         ro = np.asarray(ro, self.dt)
         B, H, W = ro.shape[:3]
@@ -596,6 +597,7 @@ class Oracle(CLib):
         p.vis_mode = 2 if scene is None else {"brute": 0, "bvh": 1, "none": 2}[vis_mode]
         p.shadow_scale = float(shadow_scale)
         p.parallel_bwd = int(parallel_bwd)
+        p.abs_terms = int(abs_terms)
         keep = [mask, ro, pos, nrm, view, kd, ks, light, pdf, rows, cols, perms]
         p.mask, p.ro, p.pos, p.nrm, p.view, p.kd, p.ks = [a.ctypes.data for a in (mask, ro, pos, nrm, view, kd, ks)]
         p.light, p.pdf, p.rows, p.cols, p.perms = [a.ctypes.data for a in (light, pdf, rows, cols, perms)]

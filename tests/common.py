@@ -152,6 +152,87 @@ def raster_mtx(kind, B, aspect=1.0):
     return np.stack(out).astype(np.float32)
 
 
+# ------------------------------------------------------------------------------------------ the per-element bar against the fp64 oracle
+N_PERT = 4
+
+
+def _ulp32(x):
+    a = np.minimum(np.abs(np.asarray(x, np.float64)), np.finfo(np.float32).max).astype(np.float32)
+    return np.nextafter(a, np.float32(np.inf)).astype(np.float64) - a.astype(np.float64)
+
+
+def _perturb(x, rng):
+    """Every element of the fp32 array x moved by one ulp up or down (seeded coin)."""
+    x = np.asarray(x, np.float32)
+    up = rng.random(x.shape) < 0.5
+    return np.where(up, np.nextafter(x, np.float32(np.inf)), np.nextafter(x, np.float32(-np.inf))).astype(np.float32)
+
+
+def check_per_element(op, got, f64, f32, ins, K, names, seed=0, exempt=None, floor=None, tag="step-tail"):
+    """got: the kernel's outputs (numpy); f64(ins) / f32(ins): the fp64 / fp32 oracle on the fp32 inputs `ins`, returning arrays of got's
+    shapes in the same order; exempt: per output, a boolean mask of elements the caller checks by another rule (or None); floor: per
+    output, a non-negative array R broadcastable to its shape (or None): the reduction floor, the most that summing the element's terms
+    in another order can change it.  With r64 / r32 the fp64 / fp32 oracle and Delta the largest change of r64 over N_PERT seeded
+    perturbations of every input element by +-1 fp32 ulp (a per-element sensitivity estimate), every finite element must satisfy
+        |got - r64| <= K * max(Delta, |r32 - r64|) + R + 4 * ulp32(r64)
+    and NaN / +-inf must sit where the fp32 oracle has them.  Returns the worst ratio (|got - r64| - R - 4 ulp) / max(Delta, |r32 - r64|)
+    over all outputs; `tag` prefixes the printed per-output line."""
+    r64 = [np.asarray(r, np.float64) for r in f64(ins)]
+    r32 = [np.asarray(r, np.float64) for r in f32(ins)]
+    rng = np.random.default_rng(1000 + seed)
+    delta = [np.zeros_like(r) for r in r64]
+    for _ in range(N_PERT):
+        for d, r, rp in zip(delta, r64, f64([_perturb(x, rng) for x in ins])):
+            np.fmax(d, np.abs(np.asarray(rp, np.float64) - r), out=d)
+    worst = 0.0
+    for k, (g, a, b, d) in enumerate(zip(got, r64, r32, delta)):
+        name = "%s: %s" % (op, names[k])
+        g = np.asarray(g, np.float64)
+        assert g.shape == a.shape, (name, g.shape, a.shape)
+        for pred, what in ((np.isnan, "NaN"), (np.isposinf, "+inf"), (np.isneginf, "-inf")):
+            bad = pred(g) != pred(b)
+            assert not bad.any(), "%s: %s at %d elements where the fp32 oracle disagrees (first %s: got %r, fp32 oracle %r)" % (
+                name, what, int(bad.sum()), tuple(np.argwhere(bad)[0]), g[bad][0], b[bad][0])
+        use = np.isfinite(g) & np.isfinite(a)
+        if exempt is not None and exempt[k] is not None:
+            use &= ~exempt[k]
+        scale = np.maximum(d, np.abs(b - a))
+        fl = 4.0 * _ulp32(a)
+        if floor is not None and floor[k] is not None:
+            fl = fl + np.nan_to_num(np.asarray(floor[k], np.float64), nan=0.0, posinf=0.0)
+        err = np.abs(g - a)
+        excess = np.maximum(err - fl, 0.0)
+        ratio = np.divide(excess, scale, out=np.where(excess > 0, np.inf, 0.0), where=scale > 0)
+        ratio = np.where(use, ratio, 0.0)
+        r = float(ratio.max()) if ratio.size else 0.0
+        worst = max(worst, r)
+        bad = use & ~(err <= K * scale + fl)
+        if bad.any():
+            idx = np.argwhere(bad)[:3]
+            fb = np.broadcast_to(fl, g.shape)
+            ex = "; ".join("%s got %.9g r64 %.9g r32 %.9g Delta %.3g floor %.3g" % (tuple(i), g[tuple(i)], a[tuple(i)], b[tuple(i)], d[tuple(i)],
+                                                                                    fb[tuple(i)]) for i in idx)
+            raise AssertionError("%s: %d of %d elements beyond %g x max(Delta, |r32 - r64|) + R + 4 ulp (worst ratio %.3g): %s" % (
+                name, int(bad.sum()), int(use.sum()), K, r, ex))
+        print("[%s] %-60s worst ratio %.3g over %d elements" % (tag, name, r, int(use.sum())))
+    return worst
+
+
+def _sample_px(B, H, W, n_rand=20000, seed=0, group=4):
+    """Flat [B*H*W] pixel indices: rows 0, 1 and H-1 of views 0 and B-1, n_rand random pixels, and the last (ragged) `group`-pixel group."""
+    n = B * H * W
+    rows = [(b * H + h) * W + np.arange(W) for b in sorted({0, B - 1}) for h in sorted({0, min(1, H - 1), H - 1})]
+    tail = np.arange(n - (n % group or group), n)
+    return np.unique(np.concatenate(rows + [np.random.default_rng(seed).integers(0, n, n_rand), tail]))
+
+
+def _take(x, grid, idx):
+    """Pixels idx of x (numpy, broadcastable to grid + (C,)) as [1,1,K,C]."""
+    x = np.asarray(x)
+    C = x.shape[-1]
+    return np.ascontiguousarray(np.broadcast_to(x, tuple(grid) + (C,)).reshape(-1, C)[idx]).reshape(1, 1, -1, C)
+
+
 def same_bits(a, b):
     """bit-for-bit equality of two fp32 arrays (so +0 / -0 and NaN payloads count)"""
     a, b = np.ascontiguousarray(a, np.float32), np.ascontiguousarray(b, np.float32)

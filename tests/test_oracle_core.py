@@ -222,3 +222,26 @@ def test_cdf_bisection_is_upper_bound():
             x = min(np.float32(x), np.float32(0.99999994))
             ub = min(int(np.searchsorted(cdf, x, side="right")), n - 1)
             assert ref(cdf, x) == ub == four_ary(cdf, x)
+
+
+@pytest.mark.parametrize("f64", [False, True])
+def test_env_shade_abs_terms_bounds_every_sum(f64):
+    """abs_terms accumulates |term| for every per-ray term: the result bounds the plain sum elementwise (rounding is monotone, so this
+    holds exactly in fp32 too), and where every term is >= 0 -- radiance and, for non-negative upstream gradients, the light gradient,
+    with a non-negative probe -- it is the plain sum itself.  The gradients of pos / nrm / ks have terms of both signs: there A is larger."""
+    o = oracle(f64)
+    c = make_case(res=16, B=1, N=4, seed=4)
+    assert (c["light"] >= 0).all()
+    args = (o.scene(c["verts"], c["tris"]), c["mask"], c["ro"], c["pos"], c["nrm"], c["view"], c["kd"], c["ks"], c["light"], c["pdf"],
+            c["rows"], c["cols"], c["perms"])
+    g = np.random.default_rng(5)
+    dg, sg = [g.uniform(0, 1, size=c["pos"].shape).astype(np.float32) for _ in range(2)]
+    kw = dict(BSDF="pbr", n_samples_x=4, rnd_seed=3, shadow_scale=0.5)
+    fwd, fwd_a = o.env_shade(*args, **kw), o.env_shade(*args, abs_terms=True, **kw)
+    bwd, bwd_a = o.env_shade(*args, grads=(dg, sg), **kw), o.env_shade(*args, grads=(dg, sg), abs_terms=True, **kw)
+    for name, r, a in zip(("diff", "spec", "pos", "nrm", "kd", "ks", "light"), fwd + bwd, fwd_a + bwd_a):
+        assert (a >= np.abs(r)).all(), name
+    for name, r, a in zip(("diff", "spec", "light"), fwd + bwd[4:], fwd_a + bwd_a[4:]):
+        assert np.array_equal(a, r) and a.max() > 0, name
+    for name, r, a in zip(("pos", "nrm", "ks"), (bwd[0], bwd[1], bwd[3]), (bwd_a[0], bwd_a[1], bwd_a[3])):
+        assert (a > np.abs(r) * 1.5).mean() > 0.05, name          # cancellation between rays: the floor is not the sum

@@ -18,6 +18,7 @@
 //   * the diffuse and specular signals, which render.py:120-121 filters with identical guides, can
 //     share one pass (NSIG = 2): weights are computed once.
 #include "common.cuh"
+#include <cfloat>          // FLT_MAX
 #include <cuda.h>          // CUtensorMap + the cuTensorMapEncodeTiled prototype (resolved at run time through cudaGetDriverEntryPoint: no libcuda link)
 
 namespace {
@@ -336,7 +337,11 @@ static int launch_bilateral(const mcs_tensor *nrm, const mcs_tensor *zdz, float 
     f.out[0] = outA; f.out[1] = outB;
     f.B = nrm->sizes[0]; f.H = nrm->sizes[1]; f.W = nrm->sizes[2];
     f.r = filter_radius(sigma);
-    f.neg_inv_2var_log2e = -LOG2E / (2.0f * sigma * sigma);
+    // Below sigma ~ 4.6e-20 the quotient overflows to -inf, and the centre tap's 0 * k2 would be NaN where the reference's -0 / (2 sigma^2)
+    // gives weight 1: -FLT_MAX keeps that 0 (every other tap's exponent is still <= -FLT_MAX, weight 0).  Only once 2 sigma^2, rounded as
+    // the reference rounds it (denoising.cu:25,53), is 0 (sigma ~ 2.6e-23) is k2 -inf, and then the reference's centre tap is NaN too.
+    const float var = sigma * sigma, two_var = 2.0f * var;
+    f.neg_inv_2var_log2e = two_var > 0.0f ? fmaxf(-LOG2E / two_var, -FLT_MAX) : -INFINITY;
     const int th = TILE_H + 2 * f.r;
     const dim3 grid((f.W + TILE_W - 1) / TILE_W, (f.H + TILE_H - 1) / TILE_H, f.B), block(32, 8, 1);
 

@@ -437,6 +437,7 @@ class Oracle(CLib):
         "orc_env_shade": ([_P], None),
         "orc_bilateral_fwd": ([_I] * 3 + [_P] * 3 + [REAL, _P], None),
         "orc_bilateral_bwd": ([_I] * 3 + [_P] * 2 + [REAL, _P, _P], None),
+        "orc_bilateral_tap_weight": ([_I] * 3 + [_P] * 2 + [REAL, _I, _I64] + [_P] * 4, None),
         "orc_det_sincos": ([_I] + [_P] * 3, None),
         "orc_det_atan2": ([_I] + [_P] * 3, None),
         "orc_det_acos": ([_I] + [_P] * 2, None),
@@ -646,6 +647,20 @@ class Oracle(CLib):
         cg = np.zeros((B, H, W, 3), self.dt)
         self.lib.orc_bilateral_bwd(B, H, W, nrm.ctypes.data, zdz.ctypes.data, sigma, out_grad.ctypes.data, cg.ctypes.data)
         return cg
+
+    def bilateral_tap_weight(self, nrm, zdz, sigma, pix, dy, dx, transposed=False):
+        """Test-only: the weight bilateral_fwd (transposed=False: the centre's depth gradient) or bilateral_bwd (transposed=True: the
+        tap's) gives the tap at pixel + (dy, dx) in the output at pixel, a flat index into [B,H,W]; exactly 0 for a tap outside the image
+        or the window.  pix, dy, dx broadcast against each other; returns an array of their shape."""
+        nrm = self._a(nrm); zdz = self._a(zdz)
+        B, H, W = nrm.shape[:3]
+        p, y, x = np.broadcast_arrays(np.asarray(pix, np.int64), np.asarray(dy, np.int32), np.asarray(dx, np.int32))
+        shape = p.shape
+        p, y, x = [np.ascontiguousarray(a).reshape(-1) for a in (p, y, x)]
+        out = np.zeros(p.shape[0], self.dt)
+        self.lib.orc_bilateral_tap_weight(B, H, W, nrm.ctypes.data, zdz.ctypes.data, sigma, int(transposed), p.shape[0], p.ctypes.data,
+                                          y.ctypes.data, x.ctypes.data, out.ctypes.data)
+        return out.reshape(shape)
 
     def bilateral_denoiser(self, col, nrm, zdz, sigma):
         """render/optixutils/ops.py:139-141"""

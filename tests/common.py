@@ -1,5 +1,7 @@
 """Shared builders for the parity tests: seeded synthetic scenes (numpy) consumable by both the CPU
 oracle and the CUDA product."""
+import ctypes as C
+import math
 import os
 import sys
 
@@ -481,3 +483,78 @@ def env_shade_edge_case():
     pdf, rows, cols = oracle().update_pdf(light)
     c.update(nrm=nrm, kd=kd, ks=ks, light=light, pdf=pdf, rows=rows, cols=cols, edge_px=px)
     return c
+
+
+# ------------------------------------------------------------------------------------------ the bilateral denoiser
+def _radius(sigma):
+    """denoising.cu:26,86: 2 * ceil(sigma * 2.5) + 1 with the product in double, sigma being an fp32 parameter."""
+    return 2 * math.ceil(float(np.float32(sigma)) * 2.5) + 1
+
+
+def _dn_both_paths(col, colB, nrm, zdz, gA, gB, sigma, dev):
+    """Raw forward [B,H,W,4] and transposed filter [B,H,W,3] through the single- and two-signal entry points, once with contiguous
+    signals (the TMA-staged kernel where the radius allows it) and once with the same values as strided views (the plain kernel).
+    All paths must agree bit for bit (NaN payloads aside); returns (forward A, forward B, backward A, backward B)."""
+    import torch
+    from nvdiffrecmc_b200 import _lib as L
+    from nvdiffrecmc_b200.optixutils.ops import _bilateral_denoiser_func, _bilateral_denoiser2_func
+    t = lambda a: torch.tensor(a, device=dev)
+    n, z = t(nrm), t(zdz)
+    wide = lambda x: torch.cat([x, torch.zeros_like(x[..., :1])], -1)[..., :x.shape[-1]]
+    res = {}
+    for tag, view in (("contiguous", lambda x: x), ("strided", wide)):
+        a, b, ga, gb = view(t(col)), view(t(colB)), view(t(gA)), view(t(gB))
+        assert a.is_contiguous() == (tag == "contiguous")
+        fa = _bilateral_denoiser_func.apply(a, n, z, sigma)
+        f2a, f2b = _bilateral_denoiser2_func.apply(a, b, n, z, sigma)
+        shape = tuple(col.shape[:3]) + (3,)
+        ca, cb, c1 = torch.empty(shape, device=dev), torch.empty(shape, device=dev), torch.empty(shape, device=dev)
+        L.check(L.lib().mcs_bilateral_bwd(C.byref(L.nhwc(n)), C.byref(L.nhwc(z)), float(sigma), C.byref(L.nhwc(ga)), c1.data_ptr(), L.stream_ptr()),
+                "bilateral_denoiser (backward)")
+        L.check(L.lib().mcs_bilateral_bwd2(C.byref(L.nhwc(n)), C.byref(L.nhwc(z)), float(sigma), C.byref(L.nhwc(ga)), C.byref(L.nhwc(gb)), ca.data_ptr(),
+                                           cb.data_ptr(), L.stream_ptr()), "bilateral_denoiser2 (backward)")
+        fa, c1 = fa.cpu().numpy(), c1.cpu().numpy()
+        res[tag] = [x.cpu().numpy() for x in (f2a, f2b, ca, cb)]
+        assert np.array_equal(nan_bits(fa), nan_bits(res[tag][0])) and np.array_equal(nan_bits(c1), nan_bits(res[tag][2])), tag
+    for k, (x, y) in enumerate(zip(res["contiguous"], res["strided"])):
+        assert np.array_equal(nan_bits(x), nan_bits(y)), "output %d: %d of %d values differ between the two kernels" % (
+            k, (nan_bits(x) != nan_bits(y)).sum(), x.size)
+    return res["contiguous"]
+
+
+def _degenerate_guides(B, H, W, seed):
+    """Piecewise-smooth guides with a zero normal inside the image, zero and negative depth gradients (each pixel is the centre of its
+    own output and a tap of its neighbours', so both uses are covered), and depth steps along x and y."""
+    rng = np.random.default_rng(seed)
+    ys, xs = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    n = np.stack([np.full((H, W), 0.2), 0.1 * np.sin(xs * 0.3), np.ones((H, W))], -1)[None] + rng.normal(size=(B, H, W, 3)) * 0.05
+    n /= np.linalg.norm(n, axis=-1, keepdims=True)
+    n[0, H // 2, W // 3] = 0.0                                    # zero centre normal
+    n[B - 1, 5, 7] = 0.0
+    z = 1.0 + xs * 0.01 + ys * 0.005 + 0.5 * (xs >= W // 2) + 0.25 * (ys >= H // 3)       # depth steps
+    z = np.broadcast_to(z, (B, H, W)) + rng.normal(size=(B, H, W)) * 1e-3
+    dz = np.abs(rng.normal(size=(B, H, W))) * 0.02 + 0.001
+    dz[0, 10:14, 20:25] = 0.0                                     # FLT_EPS guard, centre (forward) and tap (backward)
+    dz[B - 1, H // 2 - 2:H // 2 + 2, W // 2 - 3:W // 2 + 3] = -0.01   # negative gradients straddling the depth step
+    dz[0, H // 2, W // 3 + 1] = 0.0                               # next to the zero normal
+    return n.astype(np.float32), np.stack([z, dz], -1).astype(np.float32)
+
+
+def impulse_lattice(B, H, W, r, vals):
+    """The impulse lattices of the denoiser's tap-by-tap tests.  With spacing S = 2r + 1, the lattice of offset (oy, ox) holds `vals` [C]
+    at (oy + S i, ox + S j) and 0 elsewhere, so every pixel's (2r+1)^2 window holds exactly one lattice point: a filter's output there is
+    that one tap's weight times `vals` (or 0 when the point lies outside the image).  The S^2 offsets together give every in-image tap of
+    every pixel once.  Returns the lattices stacked offset-major along the batch, [S^2 B, H, W, C], and per offset, pixel of [B,H,W]:
+    (dy, dx) of that pixel's lattice point, [S^2, B, H, W] each."""
+    S = 2 * r + 1
+    vals = np.asarray(vals, np.float32)
+    sig = np.zeros((S, S, B, H, W, vals.shape[0]), np.float32)
+    for oy in range(S):
+        for ox in range(S):
+            sig[oy, ox, :, oy::S, ox::S] = vals
+    ys, xs = np.arange(H), np.arange(W)
+    dy = (np.arange(S)[:, None] - ys[None, :] + r) % S - r             # [S(oy), H]
+    dx = (np.arange(S)[:, None] - xs[None, :] + r) % S - r             # [S(ox), W]
+    DY = np.broadcast_to(dy[:, None, None, :, None], (S, S, B, H, W)).reshape(S * S, B, H, W)
+    DX = np.broadcast_to(dx[None, :, None, None, :], (S, S, B, H, W)).reshape(S * S, B, H, W)
+    return sig.reshape(S * S * B, H, W, vals.shape[0]), DY, DX

@@ -4,14 +4,11 @@ normal, roughness 0 / 1, a probe with black texels), the denoiser on degenerate 
 would round differently from the reference's double one, and the image loss at the training shape.  The fast machinery of the kernels
 (FMA contraction, the 4-pixel vector path and its scalar tail, ex2 / rsqrt approximations, env_shade's n.wi > 0 gate) is what separates
 these inputs from the easy ones of the other GPU tests; the bars are the ones the oracle meets against the reference."""
-import ctypes as C
-import math
-
 import numpy as np
 import pytest
 import torch
 
-from common import RU_OPS, env_shade_edge_case, oracle, rel_l2, ru_edge_inputs
+from common import RU_OPS, _degenerate_guides, _dn_both_paths, _radius, env_shade_edge_case, oracle, rel_l2, ru_edge_inputs
 from common import nan_bits as _bits
 
 pytestmark = pytest.mark.gpu
@@ -178,63 +175,12 @@ def test_env_shade_edge_case(dev, bsdf, shadow_scale):
 # ---------------------------------------------------------------------------------------------------------------------------------------
 # bilateral denoiser
 # ---------------------------------------------------------------------------------------------------------------------------------------
-def _radius(sigma):
-    """denoising.cu:26,86: 2 * ceil(sigma * 2.5) + 1 with the product in double, sigma being an fp32 parameter."""
-    return 2 * math.ceil(float(np.float32(sigma)) * 2.5) + 1
-
-
-def _dn_both_paths(col, colB, nrm, zdz, gA, gB, sigma, dev):
-    """Raw forward [B,H,W,4] and transposed filter [B,H,W,3] through the single- and two-signal entry points, once with contiguous
-    signals (the TMA-staged kernel where the radius allows it) and once with the same values as strided views (the plain kernel).
-    All paths must agree bit for bit; returns (forward A, forward B, backward A, backward B)."""
-    from nvdiffrecmc_b200 import _lib as L
-    from nvdiffrecmc_b200.optixutils.ops import _bilateral_denoiser_func, _bilateral_denoiser2_func
-    t = lambda a: torch.tensor(a, device=dev)
-    n, z = t(nrm), t(zdz)
-    wide = lambda x: torch.cat([x, torch.zeros_like(x[..., :1])], -1)[..., :x.shape[-1]]
-    res = {}
-    for tag, view in (("contiguous", lambda x: x), ("strided", wide)):
-        a, b, ga, gb = view(t(col)), view(t(colB)), view(t(gA)), view(t(gB))
-        assert a.is_contiguous() == (tag == "contiguous")
-        fa = _bilateral_denoiser_func.apply(a, n, z, sigma)
-        f2a, f2b = _bilateral_denoiser2_func.apply(a, b, n, z, sigma)
-        shape = tuple(col.shape[:3]) + (3,)
-        ca, cb, c1 = torch.empty(shape, device=dev), torch.empty(shape, device=dev), torch.empty(shape, device=dev)
-        L.check(L.lib().mcs_bilateral_bwd(C.byref(L.nhwc(n)), C.byref(L.nhwc(z)), float(sigma), C.byref(L.nhwc(ga)), c1.data_ptr(), L.stream_ptr()),
-                "bilateral_denoiser (backward)")
-        L.check(L.lib().mcs_bilateral_bwd2(C.byref(L.nhwc(n)), C.byref(L.nhwc(z)), float(sigma), C.byref(L.nhwc(ga)), C.byref(L.nhwc(gb)), ca.data_ptr(),
-                                           cb.data_ptr(), L.stream_ptr()), "bilateral_denoiser2 (backward)")
-        assert torch.equal(fa, f2a) and torch.equal(c1, ca), tag
-        res[tag] = [x.cpu().numpy() for x in (f2a, f2b, ca, cb)]
-    for k, (x, y) in enumerate(zip(res["contiguous"], res["strided"])):
-        assert np.array_equal(x, y), "output %d: %d of %d values differ between the two kernels" % (k, (x != y).sum(), x.size)
-    return res["contiguous"]
-
-
 def _dn_check_oracle(col, colB, nrm, zdz, gA, gB, sigma, outs):
     o = oracle()
     for k, (got, want) in enumerate(zip(outs, (o.bilateral_fwd(col, nrm, zdz, sigma), o.bilateral_fwd(colB, nrm, zdz, sigma),
                                                o.bilateral_bwd(nrm, zdz, sigma, gA), o.bilateral_bwd(nrm, zdz, sigma, gB)))):
         assert np.isfinite(got).all(), k
         assert rel_l2(got, want) < 1e-4, (k, rel_l2(got, want))
-
-
-def _degenerate_guides(B, H, W, seed):
-    """Piecewise-smooth guides with a zero normal inside the image, zero and negative depth gradients (each pixel is the centre of its
-    own output and a tap of its neighbours', so both uses are covered), and depth steps along x and y."""
-    rng = np.random.default_rng(seed)
-    ys, xs = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
-    n = np.stack([np.full((H, W), 0.2), 0.1 * np.sin(xs * 0.3), np.ones((H, W))], -1)[None] + rng.normal(size=(B, H, W, 3)) * 0.05
-    n /= np.linalg.norm(n, axis=-1, keepdims=True)
-    n[0, H // 2, W // 3] = 0.0                                    # zero centre normal
-    n[B - 1, 5, 7] = 0.0
-    z = 1.0 + xs * 0.01 + ys * 0.005 + 0.5 * (xs >= W // 2) + 0.25 * (ys >= H // 3)       # depth steps
-    z = np.broadcast_to(z, (B, H, W)) + rng.normal(size=(B, H, W)) * 1e-3
-    dz = np.abs(rng.normal(size=(B, H, W))) * 0.02 + 0.001
-    dz[0, 10:14, 20:25] = 0.0                                     # FLT_EPS guard, centre (forward) and tap (backward)
-    dz[B - 1, H // 2 - 2:H // 2 + 2, W // 2 - 3:W // 2 + 3] = -0.01   # negative gradients straddling the depth step
-    dz[0, H // 2, W // 3 + 1] = 0.0                               # next to the zero normal
-    return n.astype(np.float32), np.stack([z, dz], -1).astype(np.float32)
 
 
 @pytest.mark.parametrize("sigma", [0.6, 2.0, 3.0])

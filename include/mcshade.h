@@ -379,6 +379,32 @@ int mcs_sdf_reg_fwd(const float *sdf, int64_t sdf_stride, const int32_t *edges, 
 int mcs_sdf_reg_bwd(const float *sdf, int64_t sdf_stride, int32_t V, const int32_t *edges, const int32_t *v2e_offsets, const int32_t *v2e_edges,
                     const float *m, const float *d_loss, float *d_sdf, mcs_stream stream);
 
+/* ---- image-space regularisers: shading_loss, material_smoothness_grad and chroma_loss (render/regularizer.py:15-49); semantics, and the
+ *      torch conventions they keep (ties of max, clamp boundaries, abs at 0, the sRGB branch, the means' denominators), in
+ *      csrc/regularizer.cu.  Every operand is an fp32 [B,H,W,4] view with any non-negative element strides; all operands of one call have
+ *      the same B, H and W, and B*H*W < 2^31.  lambda_* by value (the fp32 rounding of the reference's Python float).
+ *      _fwd writes the loss (one float on the device) through `partials`: mcs_<name>_num_partials(B,H,W) x K doubles of device scratch,
+ *      K = 3 for shading_loss and material_smoothness_grad, 1 for chroma_loss; the sums are fixed-order, so two runs give the same bits.
+ *      shading_loss_fwd also writes means (two floats on the device) = (mean of diffuse luma, mean of specular luma), which its backward
+ *      reads.  _bwd reads the upstream gradient d_loss (one float on the device) and overwrites the dense, contiguous [B,H,W,4] gradients
+ *      (16-byte aligned) of every rendered operand, alpha included; chroma_loss's kd gradient has alpha 0, shading_loss's light gradients
+ *      have alpha 0.  color_ref is a constant.  No entry synchronises the host. */
+int32_t mcs_shading_loss_num_partials(int32_t B, int32_t H, int32_t W);
+int mcs_shading_loss_fwd(const mcs_tensor *diffuse_light, const mcs_tensor *specular_light, const mcs_tensor *color_ref, float lambda_diffuse,
+                         float lambda_specular, double *partials, float *loss, float *means, mcs_stream stream);
+int mcs_shading_loss_bwd(const mcs_tensor *diffuse_light, const mcs_tensor *specular_light, const mcs_tensor *color_ref, float lambda_diffuse,
+                         float lambda_specular, const float *means, const float *d_loss, float *d_diffuse_light, float *d_specular_light,
+                         mcs_stream stream);
+int32_t mcs_material_smoothness_grad_num_partials(int32_t B, int32_t H, int32_t W);
+int mcs_material_smoothness_grad_fwd(const mcs_tensor *kd_grad, const mcs_tensor *ks_grad, const mcs_tensor *nrm_grad, float lambda_kd,
+                                     float lambda_ks, float lambda_nrm, double *partials, float *loss, mcs_stream stream);
+int mcs_material_smoothness_grad_bwd(const mcs_tensor *kd_grad, const mcs_tensor *ks_grad, const mcs_tensor *nrm_grad, float lambda_kd,
+                                     float lambda_ks, float lambda_nrm, const float *d_loss, float *d_kd_grad, float *d_ks_grad,
+                                     float *d_nrm_grad, mcs_stream stream);
+int32_t mcs_chroma_loss_num_partials(int32_t B, int32_t H, int32_t W);
+int mcs_chroma_loss_fwd(const mcs_tensor *kd, const mcs_tensor *color_ref, float lambda_chroma, double *partials, float *loss, mcs_stream stream);
+int mcs_chroma_loss_bwd(const mcs_tensor *kd, const mcs_tensor *color_ref, float lambda_chroma, const float *d_loss, float *d_kd, mcs_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

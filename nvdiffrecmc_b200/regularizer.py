@@ -1,0 +1,164 @@
+"""The image-space regularisers of both geometry passes on the GPU: drop-ins for the reference's `shading_loss`,
+`material_smoothness_grad` and `chroma_loss` (render/regularizer.py:15-49), run by the kernels of csrc/regularizer.cu (contract stated
+there: torch's conventions for ties of max, clamp boundaries, abs at 0, the sRGB branch and the means' denominators).
+
+Each function returns a 0-dim fp32 device tensor, as `torch.mean(...) * lambda` does.  Forward and backward are one streaming launch
+each (plus a one-CTA finish in the forward), make no host synchronisation and can be captured in a CUDA graph; the backward reads its
+upstream gradient from the device.  Gradients flow to every rendered operand, all four channels (alpha comes from the composite and
+depends on the geometry); `kd`'s alpha gets exactly 0 and `color_ref` is the constant target.
+
+Operands are fp32 CUDA [B,H,W,4] tensors of one shape, with any strides (`color_ref` is often a slice).  A wrong channel count, a shape
+mismatch, a CPU tensor, a non-float lambda or a `color_ref` that requires grad raises ValueError before anything is launched.
+"""
+import torch
+
+from . import _lib as L
+
+__all__ = ["shading_loss", "material_smoothness_grad", "chroma_loss"]
+
+
+def _check(fn, named, lambdas):
+    """ValueError naming the argument unless every (name, tensor) of `named` is an fp32 CUDA [B,H,W,4] tensor of the first one's shape on
+    its device, every (name, value) of `lambdas` is a Python float, and color_ref (if given) does not require grad."""
+    first_name, first = named[0]
+    for name, t in named:
+        if not isinstance(t, torch.Tensor):
+            raise ValueError("%s: %s must be a torch.Tensor, got %s" % (fn, name, type(t).__name__))
+        if t.dtype != torch.float32:
+            raise ValueError("%s: %s must be float32, got %s" % (fn, name, t.dtype))
+        if t.dim() != 4 or t.shape[3] != 4:
+            raise ValueError("%s: %s must be [B,H,W,4], got %s" % (fn, name, tuple(t.shape)))
+        if not t.is_cuda:
+            raise ValueError("%s: %s must be a CUDA tensor, got %s" % (fn, name, t.device))
+        if t.shape != first.shape:
+            raise ValueError("%s: %s has shape %s, %s has %s" % (fn, name, tuple(t.shape), first_name, tuple(first.shape)))
+        if t.device != first.device:
+            raise ValueError("%s: %s is on %s, %s on %s" % (fn, name, t.device, first_name, first.device))
+        if t.numel() == 0:
+            raise ValueError("%s: %s is empty" % (fn, name))
+        if any(s >= 2 ** 31 for s in t.stride()):
+            raise ValueError("%s: %s has a stride beyond int32" % (fn, name))
+        if name == "color_ref" and t.requires_grad:
+            raise ValueError("%s: color_ref is the constant target and must not require grad" % fn)
+    if first.shape[0] * first.shape[1] * first.shape[2] >= 2 ** 31:
+        raise ValueError("%s: at most 2^31 - 1 pixels" % fn)
+    for name, v in lambdas:
+        if not isinstance(v, float):
+            raise ValueError("%s: %s must be a float, got %s" % (fn, name, type(v).__name__))
+
+
+def _partials(fn, t, k):
+    B, H, W = t.shape[:3]
+    return torch.empty(k * getattr(L.lib(), "mcs_%s_num_partials" % fn)(B, H, W), dtype=torch.float64, device=t.device)
+
+
+def _grad(t):
+    return torch.empty(t.shape, dtype=torch.float32, device=t.device)
+
+
+def _upstream(d_loss):
+    return d_loss.to(torch.float32).contiguous()
+
+
+# ---- shading_loss ----
+def _shading_fwd(d, s, r, ld, ls):
+    loss = torch.empty((), dtype=torch.float32, device=d.device)
+    means = torch.empty(2, dtype=torch.float32, device=d.device)
+    L.check(L.lib().mcs_shading_loss_fwd(L.nhwc(d), L.nhwc(s), L.nhwc(r), ld, ls, _partials("shading_loss", d, 3).data_ptr(), loss.data_ptr(),
+                                         means.data_ptr(), L.stream_ptr()), "shading_loss_fwd")
+    return loss, means
+
+
+class _ShadingLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, d, s, r, ld, ls):
+        loss, means = _shading_fwd(d, s, r, ld, ls)
+        ctx.save_for_backward(d, s, r, means)
+        ctx.lambdas = (ld, ls)
+        return loss
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        d, s, r, means = ctx.saved_tensors
+        gd, gs = _grad(d), _grad(s)
+        L.check(L.lib().mcs_shading_loss_bwd(L.nhwc(d), L.nhwc(s), L.nhwc(r), *ctx.lambdas, means.data_ptr(), _upstream(d_loss).data_ptr(),
+                                             gd.data_ptr(), gs.data_ptr(), L.stream_ptr()), "shading_loss_bwd")
+        return (gd if ctx.needs_input_grad[0] else None), (gs if ctx.needs_input_grad[1] else None), None, None, None
+
+
+def shading_loss(diffuse_light, specular_light, color_ref, lambda_diffuse, lambda_specular):
+    """The reference's monochrome shading regulariser: the log-sRGB error of the lights' luma against color_ref's value, weighted by the
+    diffuse share, plus mean specular luma over mean diffuse luma.  -> 0-dim fp32 tensor, differentiable in both lights."""
+    _check("shading_loss", [("diffuse_light", diffuse_light), ("specular_light", specular_light), ("color_ref", color_ref)],
+           [("lambda_diffuse", lambda_diffuse), ("lambda_specular", lambda_specular)])
+    if torch.is_grad_enabled() and (diffuse_light.requires_grad or specular_light.requires_grad):
+        return _ShadingLoss.apply(diffuse_light, specular_light, color_ref, lambda_diffuse, lambda_specular)
+    return _shading_fwd(diffuse_light.detach(), specular_light.detach(), color_ref, lambda_diffuse, lambda_specular)[0]
+
+
+# ---- material_smoothness_grad ----
+def _smooth_fwd(k, s, n, lam):
+    loss = torch.empty((), dtype=torch.float32, device=k.device)
+    L.check(L.lib().mcs_material_smoothness_grad_fwd(L.nhwc(k), L.nhwc(s), L.nhwc(n), *lam, _partials("material_smoothness_grad", k, 3).data_ptr(),
+                                                     loss.data_ptr(), L.stream_ptr()), "material_smoothness_grad_fwd")
+    return loss
+
+
+class _MaterialSmoothness(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, k, s, n, lkd, lks, lnrm):
+        ctx.save_for_backward(k, s, n)
+        ctx.lambdas = (lkd, lks, lnrm)
+        return _smooth_fwd(k, s, n, ctx.lambdas)
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        k, s, n = ctx.saved_tensors
+        gk, gs, gn = _grad(k), _grad(s), _grad(n)
+        L.check(L.lib().mcs_material_smoothness_grad_bwd(L.nhwc(k), L.nhwc(s), L.nhwc(n), *ctx.lambdas, _upstream(d_loss).data_ptr(),
+                                                         gk.data_ptr(), gs.data_ptr(), gn.data_ptr(), L.stream_ptr()),
+                "material_smoothness_grad_bwd")
+        return tuple(g if need else None for g, need in zip((gk, gs, gn), ctx.needs_input_grad[:3])) + (None, None, None)
+
+
+def material_smoothness_grad(kd_grad, ks_grad, nrm_grad, lambda_kd=0.25, lambda_ks=0.1, lambda_nrm=0.0):
+    """The reference's material smoothness regulariser over the jittered-tap differences kd_grad, ks_grad, nrm_grad (rgb, coverage
+    alpha).  -> 0-dim fp32 tensor, differentiable in all four channels of each."""
+    _check("material_smoothness_grad", [("kd_grad", kd_grad), ("ks_grad", ks_grad), ("nrm_grad", nrm_grad)],
+           [("lambda_kd", lambda_kd), ("lambda_ks", lambda_ks), ("lambda_nrm", lambda_nrm)])
+    if torch.is_grad_enabled() and (kd_grad.requires_grad or ks_grad.requires_grad or nrm_grad.requires_grad):
+        return _MaterialSmoothness.apply(kd_grad, ks_grad, nrm_grad, lambda_kd, lambda_ks, lambda_nrm)
+    return _smooth_fwd(kd_grad.detach(), ks_grad.detach(), nrm_grad.detach(), (lambda_kd, lambda_ks, lambda_nrm))
+
+
+# ---- chroma_loss ----
+def _chroma_fwd(k, r, lc):
+    loss = torch.empty((), dtype=torch.float32, device=k.device)
+    L.check(L.lib().mcs_chroma_loss_fwd(L.nhwc(k), L.nhwc(r), lc, _partials("chroma_loss", k, 1).data_ptr(), loss.data_ptr(), L.stream_ptr()),
+            "chroma_loss_fwd")
+    return loss
+
+
+class _ChromaLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, k, r, lc):
+        ctx.save_for_backward(k, r)
+        ctx.lc = lc
+        return _chroma_fwd(k, r, lc)
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        k, r = ctx.saved_tensors
+        gk = _grad(k)
+        L.check(L.lib().mcs_chroma_loss_bwd(L.nhwc(k), L.nhwc(r), ctx.lc, _upstream(d_loss).data_ptr(), gk.data_ptr(), L.stream_ptr()),
+                "chroma_loss_bwd")
+        return gk, None, None
+
+
+def chroma_loss(kd, color_ref, lambda_chroma):
+    """The reference's chroma regulariser: |kd / value(kd) - color_ref / value(color_ref)| where color_ref covers, over rgb.  -> 0-dim
+    fp32 tensor, differentiable in kd's rgb (kd's alpha gets 0)."""
+    _check("chroma_loss", [("kd", kd), ("color_ref", color_ref)], [("lambda_chroma", lambda_chroma)])
+    if torch.is_grad_enabled() and kd.requires_grad:
+        return _ChromaLoss.apply(kd, color_ref, lambda_chroma)
+    return _chroma_fwd(kd.detach(), color_ref, lambda_chroma)

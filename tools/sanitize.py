@@ -90,5 +90,11 @@ dat = (torch.randn(2, 9, 11, 4, device=dev) * 0.2).requires_grad_(True)
 texture(torch.rand(2, 5, 7, 3, device=dev, requires_grad=True), uvt, filter_mode="linear", boundary_mode="clamp").sum().backward()
 mipc = [torch.rand(1, max(1, 12 >> k), max(1, 20 >> k), 4, device=dev, requires_grad=True) for k in range(5)]
 texture(mipc[0], uvt, dat, mip=mipc[1:]).sum().backward()
+# image-space regularisers: a ragged pixel count (one partial CTA), a strided color_ref slice and a strided kd_grad, forward + backward
+import nvdiffrecmc_b200.regularizer as reg
+rb = torch.rand(2, 9, 11, 8, device=dev)
+lights = [torch.rand(2, 9, 11, 4, device=dev, requires_grad=True) for _ in range(2)]
+(reg.shading_loss(*lights, rb[..., 2:6], 0.15, 0.0025) + reg.chroma_loss(lights[0], rb[..., 2:6], 0.025)).backward()
+reg.material_smoothness_grad(torch.rand(2, 9, 11, 8, device=dev)[..., 1:5].requires_grad_(True), lights[0], lights[1], 0.1, 0.05, 0.025).backward()
 torch.cuda.synchronize()
 print("sanitize workload ok", float(loss), int(v.sum()), tuple(pts.shape))

@@ -347,6 +347,21 @@ int mcs_texture_fwd(const mcs_texture_levels *tex, const float *uv, const float 
 int mcs_texture_bwd(const mcs_texture_levels *tex, const float *uv, const float *uv_da, int32_t B, int32_t H, int32_t W, int32_t filter_mode,
                     int32_t boundary_mode, const float *d_out, float *const *d_tex, float *d_uv, float *d_uv_da, mcs_stream stream);
 
+/* ---- Texture2D's automatic mip chain (render/texture.py:20-30,57-68) and its in-place clamp_ / normalize_ (texture.py:89-100); semantics
+ *      in csrc/texture.cu.  Level tables as above, every level [Bt, h[k], w[k], C] fp32 contiguous with batch_stride[k] = h*w*C (or 0 when
+ *      Bt = 1).  A chain table (_chain_fwd / _chain_bwd, 2..16 levels) has the 2 x 2 pool's sizes, h[k] = h[k-1] / 2 with h[k-1] >= 2 and
+ *      w alike; clamp and normalize take any table of the sampling layout (custom chains included).
+ *      mcs_mip_chain_fwd reads level 0 and overwrites levels 1..n-1 (the table's pointers are written through); it takes
+ *      mcs_mip_chain_fwd_launches(n_levels) launches.  mcs_mip_chain_bwd reads the incoming gradient of each level (ptr[k], null = zero; at
+ *      least one given) and overwrites d_base [Bt, h[0], w[0], C] with the gradient of level 0; one launch, no atomics.
+ *      mcs_mip_clamp clamps every level in place per channel to [lo[c], hi[c]] (device fp32 arrays of >= C entries); mcs_mip_normalize
+ *      (C = 3) normalises every texel of every level in place; one launch each.  No entry allocates or synchronises the host. */
+int32_t mcs_mip_chain_fwd_launches(int32_t n_levels);
+int mcs_mip_chain_fwd(const mcs_texture_levels *chain, int32_t Bt, mcs_stream stream);
+int mcs_mip_chain_bwd(const mcs_texture_levels *grads, int32_t Bt, float *d_base, mcs_stream stream);
+int mcs_mip_clamp(const mcs_texture_levels *levels, int32_t Bt, const float *lo, const float *hi, mcs_stream stream);
+int mcs_mip_normalize(const mcs_texture_levels *levels, int32_t Bt, mcs_stream stream);
+
 /* ---- DMTet geometry: marching_tets and sdf_reg_loss (geometry/dmtet.py:91-153); semantics in csrc/dmtet.cu.  All arrays are device
  *      memory.  Static tables of one tet grid (V vertices, T tets, E unique edges), built once by the caller:
  *        edges [E,2] int32, 8-byte aligned: the unique vertex pairs of the tets' six base edges, each as (min, max), sorted

@@ -9,6 +9,7 @@ Sub-packages mirror the reference layout:
     nvdiffrecmc_b200.light        <->  render/light.py      (EnvironmentLight)
     nvdiffrecmc_b200.dmtet        <->  geometry/dmtet.py    (marching_tets, sdf_reg_loss)
     nvdiffrecmc_b200.regularizer  <->  render/regularizer.py (shading_loss, material_smoothness_grad, chroma_loss)
+    nvdiffrecmc_b200.texture      <->  render/texture.py    (Texture2D: its automatic mip chain, clamp_, normalize_)
 All of them call hand-written CUDA kernels in lib/libmcshade.so through the C ABI in include/mcshade.h.
 """
 from . import _lib  # noqa: F401

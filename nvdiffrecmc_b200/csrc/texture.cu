@@ -36,6 +36,26 @@
 // Every operation above is explicitly rounded (__fmul_rn / __fadd_rn / __fsub_rn / __fdiv_rn / __fsqrt_rn, never contracted), so the
 // forward, d uv and d uv_da are bit-reproducible against the fp32 oracle.  No hardware texture filtering: its 8-bit fixed-point weights
 // would break the contract.
+//
+// Texture2D's automatic mip chain (render/texture.py:20-30,57-68) and its in-place updates (texture.py:89-100), on level tables of the
+// same layout, every level [Bt, h_k, w_k, C] fp32 contiguous (the CPU oracle oracle/mipchain.c restates this part):
+//   Chain forward: levels 1..L of level 0, h_k = h_0 >> k, w_k = w_0 >> k (the chain stops as soon as either side is 1, so every pooled
+//     level has both sides >= 2); texel (y, x) of level k+1 = ((((0 + t[2y,2x]) + t[2y,2x+1]) + t[2y+1,2x]) + t[2y+1,2x+1]) / 4 of level k,
+//     rounded at each step: avg_pool2d((2, 2))'s float accumulation, row-major; an odd side drops its last row or column.  A CTA pools a
+//     32 x 32 tile of level s through levels s+1 .. s+5 in shared memory (level s+j of the tile depends on that tile only), so a chain of
+//     L levels takes ceil(L / 5) launches: two for 1024^2 (L = 10).
+//   Chain backward (the fold): d level 0 = D_0, where D_top = G_top for the coarsest level `top` with an incoming gradient and
+//     D_k = G_k + U(0.25 * D_{k+1}) below it (an absent G_k is zero: D_k = U(...)).  U is the clamped bilinear tap above, in its
+//     operation order, of level k+1 at the centres of level k's texels: the exact coordinate x = i / 2 - 0.25 gives x0 = floor(x) clamped,
+//     fx = 0.75 (i even) or 0.25 (i odd), and 0.25 * D is rounded once per texel before the blend.  For power-of-two sides this is the
+//     grid of the reference's torch.linspace, so the arithmetic is the reference's bit for bit; for other sides linspace's own rounding
+//     moves the reference's weights by an ulp, the one intended difference.  One launch, no atomics: a CTA owns a 32 x 32 tile of level 0
+//     and recomputes, from the coarsest live level down, the few texels of each coarser level that tile reads (at most 18 x 18 at level 1,
+//     a handful above), so every D_0 texel is evaluated in one fixed order and two runs give the same bits.
+//   Clamp: x = min(max(x, lo[c]), hi[c]) per channel over every level, as torch.clamp with tensor bounds: a NaN texel stays NaN, else a
+//     NaN bound is returned; lo / hi are read on the device.  One launch.
+//   Normalize (C = 3): x / sqrt(max(dot(x, x), 1e-20)) per texel over every level (util.safe_normalize); dot left to right, NaN kept
+//     through the max.  One launch.
 #include "common.cuh"
 
 // Layout choices, measured with tools/texbench.py on bench.py's shape (8 x 512^2, Texture2D.sample x 3 on 1024^2 chains and the five
@@ -110,9 +130,9 @@ __device__ __forceinline__ Lod tex_lod(const float4 da, float W0, float H0, int 
 // the four taps of one level: element offsets of t00, t10, t01, t11 (texel * C + minibatch offset) and the bilinear fractions
 struct Taps { int64_t o00, o10, o01, o11; float fx, fy; };
 
-__device__ __forceinline__ void tex_axis(float u, int n, bool clamp, int &i0, int &i1, float &fr)
+// one axis of the taps at texel-space coordinate x (texel centres at integer + 0.5 - 0.5 = integers)
+__device__ __forceinline__ void tex_axis_at(float x, int n, bool clamp, int &i0, int &i1, float &fr)
 {
-    const float x = __fsub_rn(__fmul_rn(u, (float)n), 0.5f);
     fr = __fsub_rn(x, floorf(x));
     const int x0 = __float2int_rd(x);                  // cvt.rmi.s32.f32: saturating, NaN -> 0
     if (clamp) {
@@ -123,6 +143,11 @@ __device__ __forceinline__ void tex_axis(float u, int n, bool clamp, int &i0, in
         if (i0 < 0) i0 += n;
         i1 = i0 + 1 == n ? 0 : i0 + 1;
     }
+}
+
+__device__ __forceinline__ void tex_axis(float u, int n, bool clamp, int &i0, int &i1, float &fr)
+{
+    tex_axis_at(__fsub_rn(__fmul_rn(u, (float)n), 0.5f), n, clamp, i0, i1, fr);
 }
 
 __device__ __forceinline__ Taps tex_taps(const mcs_texture_levels &lv, int k, int b, float u, float v, bool clamp)
@@ -404,6 +429,189 @@ int tex_launch(const TexArgs &a, cudaStream_t s, bool bwd)
     return 0;
 }
 
+// ---- mip chain: forward, fold, clamp, normalize -------------------------------------------------------------------------------------
+
+constexpr int MIP_STEPS = 5;                 // levels per chain-forward launch: a 32 x 32 tile pools down to one texel
+constexpr int MIP_CH = 4;                    // channels per pass through shared memory
+constexpr int FOLD_TILE = 32;                // level-0 texels per fold CTA side
+constexpr int FOLD_REG = FOLD_TILE / 2 + 2;  // largest side of the region a fold tile reads at level >= 1 (level 1; coarser ones shrink)
+
+__device__ __forceinline__ float pool4(float t00, float t01, float t10, float t11)
+{
+    return __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fadd_rn(0.0f, t00), t01), t10), t11), 4.0f);
+}
+
+__device__ __forceinline__ float *level_ptr(const mcs_texture_levels &lv, int k, int b)
+{
+    return const_cast<float *>(lv.ptr[k]) + (int64_t)b * lv.batch_stride[k];
+}
+
+// levels s+1 .. s+n (n <= MIP_STEPS) of the 32 x 32 tile (blockIdx.x, blockIdx.y) of level s, minibatch blockIdx.z.  Thread i of a pass
+// owns (texel i / cc, channel i % cc) of a 16 x 16 level-(s+1) tile; level s+j of the tile is ping-ponged through shared memory.
+__global__ void __launch_bounds__(256) k_mip_down(const mcs_texture_levels lv, int s, int n)
+{
+    __shared__ float buf[2][16 * 16 * MIP_CH];
+    const int b = blockIdx.z, C = lv.C;
+    for (int c0 = 0; c0 < C; c0 += MIP_CH) {
+        const int cc = min(MIP_CH, C - c0);
+        for (int j = 1; j <= n; ++j) {
+            const int side = 16 >> (j - 1), k = s + j, H = lv.h[k], W = lv.w[k];
+            const float *prev = buf[(j - 2) & 1];
+            float *cur = buf[(j - 1) & 1];
+            float *dst = level_ptr(lv, k, b);
+            const float *src = level_ptr(lv, s, b);
+            const int64_t Ws = lv.w[s];
+            for (int i = threadIdx.x; i < side * side * cc; i += blockDim.x) {
+                const int c = i % cc, r = i / cc, ty = r / side, tx = r % side;
+                const int y = blockIdx.y * side + ty, x = blockIdx.x * side + tx;
+                float v = 0.0f;
+                if (y < H && x < W) {
+                    if (j == 1) {
+                        const float *p = src + ((2 * y) * Ws + 2 * x) * C + c0 + c;
+                        v = pool4(p[0], p[C], p[Ws * C], p[Ws * C + C]);
+                    } else {
+                        const float *p = prev + ((2 * ty) * (2 * side) + 2 * tx) * MIP_CH + c;
+                        v = pool4(p[0], p[MIP_CH], p[2 * side * MIP_CH], p[2 * side * MIP_CH + MIP_CH]);
+                    }
+                    dst[((int64_t)y * W + x) * C + c0 + c] = v;
+                }
+                cur[r * MIP_CH + c] = v;             // texels outside the level are never read: their parents are outside too
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// coarse coordinate of fine texel i under the 2 x 2 pool: i / 2 - 0.25, exact
+__device__ __forceinline__ float fold_coord(int i) { return __fsub_rn(__fmul_rn((float)i, 0.5f), 0.25f); }
+
+// D_k at (y, x, channel ch) of minibatch b; `up` holds D_{k+1} over the region (uy, ux, unx wide) when k < top
+__device__ __forceinline__ float fold_texel(const mcs_texture_levels &g, int k, int top, int b, int y, int x, int ch, int c, const float *up,
+                                            int uy, int ux, int unx)
+{
+    float s = 0.0f;
+    if (k < top) {
+        int y0, y1, x0, x1;
+        float fy, fx;
+        tex_axis_at(fold_coord(y), g.h[k + 1], true, y0, y1, fy);
+        tex_axis_at(fold_coord(x), g.w[k + 1], true, x0, x1, fx);
+        const auto t = [&](int yy, int xx) { return __fmul_rn(0.25f, up[((yy - uy) * unx + (xx - ux)) * MIP_CH + c]); };
+        s = bilerp(t(y0, x0), t(y0, x1), t(y1, x0), t(y1, x1), fx, fy);
+    }
+    if (g.ptr[k] == nullptr) return s;
+    const float gk = g.ptr[k][(int64_t)b * g.batch_stride[k] + ((int64_t)y * g.w[k] + x) * g.C + ch];
+    return k < top ? __fadd_rn(gk, s) : gk;
+}
+
+__global__ void __launch_bounds__(256) k_mip_fold(const mcs_texture_levels g, int top, float *d0)
+{
+    __shared__ float buf[2][FOLD_REG * FOLD_REG * MIP_CH];
+    __shared__ int lo_y[16], lo_x[16], n_y[16], n_x[16];
+    const int b = blockIdx.z, C = g.C;
+    if (threadIdx.x == 0) {
+        int ly = blockIdx.y * FOLD_TILE, lx = blockIdx.x * FOLD_TILE, hy = min(ly + FOLD_TILE, g.h[0]) - 1, hx = min(lx + FOLD_TILE, g.w[0]) - 1;
+        for (int k = 0; k <= top; ++k) {
+            if (k > 0) {          // the taps of fine rows lo..hi: coarse rows (lo - 1) >> 1 .. (hi + 1) >> 1, clamped
+                ly = max(0, (ly - 1) >> 1); hy = min(g.h[k] - 1, (hy + 1) >> 1);
+                lx = max(0, (lx - 1) >> 1); hx = min(g.w[k] - 1, (hx + 1) >> 1);
+            }
+            lo_y[k] = ly; lo_x[k] = lx; n_y[k] = hy - ly + 1; n_x[k] = hx - lx + 1;
+        }
+    }
+    __syncthreads();
+    for (int c0 = 0; c0 < C; c0 += MIP_CH) {
+        const int cc = min(MIP_CH, C - c0);
+        for (int k = top; k >= 0; --k) {
+            const float *up = buf[(k + 1) & 1];
+            float *cur = buf[k & 1];
+            const int nx = n_x[k], uy = k < top ? lo_y[k + 1] : 0, ux = k < top ? lo_x[k + 1] : 0, unx = k < top ? n_x[k + 1] : 0;
+            for (int i = threadIdx.x; i < n_y[k] * nx * cc; i += blockDim.x) {
+                const int c = i % cc, r = i / cc, y = lo_y[k] + r / nx, x = lo_x[k] + r % nx;
+                const float v = fold_texel(g, k, top, b, y, x, c0 + c, c, up, uy, ux, unx);
+                if (k > 0) cur[r * MIP_CH + c] = v;
+                else d0[(((int64_t)b * g.h[0] + y) * g.w[0] + x) * C + c0 + c] = v;
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// one flat index over every level's elements (per = C) or texels (per = 1)
+struct MipFlat { int64_t end[16]; };
+
+__device__ __forceinline__ int flat_level(const MipFlat &f, int64_t i, int64_t &j)
+{
+    int k = 0;
+    while (i >= f.end[k]) ++k;
+    j = i - (k ? f.end[k - 1] : 0);
+    return k;
+}
+
+__global__ void __launch_bounds__(256) k_mip_clamp(const mcs_texture_levels lv, const MipFlat f, int n, const float *lo, const float *hi)
+{
+    const int64_t total = f.end[n - 1];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        int64_t j;
+        float *p = const_cast<float *>(lv.ptr[flat_level(f, i, j)]) + j;
+        const int c = (int)(j % lv.C);
+        const float x = *p, l = __ldg(lo + c), h = __ldg(hi + c);
+        if (x != x) continue;
+        *p = l != l ? l : (h != h ? h : fminf(fmaxf(x, l), h));
+    }
+}
+
+__global__ void __launch_bounds__(256) k_mip_normalize(const mcs_texture_levels lv, const MipFlat f, int n)
+{
+    const int64_t total = f.end[n - 1];
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+        int64_t j;
+        float *p = const_cast<float *>(lv.ptr[flat_level(f, i, j)]) + 3 * j;
+        const float x = p[0], y = p[1], z = p[2];
+        const float d = __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
+        const float l = __fsqrt_rn(d != d ? d : fmaxf(d, 1e-20f));
+        p[0] = __fdiv_rn(x, l); p[1] = __fdiv_rn(y, l); p[2] = __fdiv_rn(z, l);
+    }
+}
+
+// A level table of one chain: `pooled` asks for the 2 x 2 pool's sizes (h_k = h_{k-1} / 2 with h_{k-1} >= 2, w alike), else the
+// sampling table's h_k = max(1, h_0 >> k); `null_ok` lets levels be absent (the fold's gradients).
+int mip_validate(const char *fn, const mcs_texture_levels *lv, int32_t Bt, int min_levels, bool pooled, bool null_ok)
+{
+    MCS_REQUIRE(lv != nullptr, "%s: null pointer (level table)", fn);
+    MCS_REQUIRE(lv->n_levels >= min_levels && lv->n_levels <= 16, "%s: n_levels must be in %d..16 (got %d)", fn, min_levels, lv->n_levels);
+    MCS_REQUIRE(lv->C >= 1, "%s: C must be >= 1 (got %d)", fn, lv->C);
+    MCS_REQUIRE(Bt >= 1 && Bt <= 65535, "%s: Bt must be in 1..65535 (got %d)", fn, Bt);
+    MCS_REQUIRE(lv->h[0] >= 1 && lv->w[0] >= 1 && lv->h[0] <= (1 << 20) && lv->w[0] <= (1 << 20), "%s: level 0 is %d x %d (each side 1..2^20)", fn,
+                lv->h[0], lv->w[0]);
+    bool any = false;
+    for (int k = 0; k < lv->n_levels; ++k) {
+        MCS_REQUIRE(null_ok || lv->ptr[k] != nullptr, "%s: null pointer (level %d)", fn, k);
+        any |= lv->ptr[k] != nullptr;
+        if (k > 0 && pooled)
+            MCS_REQUIRE(lv->h[k - 1] >= 2 && lv->w[k - 1] >= 2 && lv->h[k] == lv->h[k - 1] / 2 && lv->w[k] == lv->w[k - 1] / 2,
+                        "%s: level %d is %d x %d, which is not the 2 x 2 pool of level %d (%d x %d)", fn, k, lv->h[k], lv->w[k], k - 1,
+                        lv->h[k - 1], lv->w[k - 1]);
+        if (k > 0 && !pooled)
+            MCS_REQUIRE(lv->h[k] == max(1, lv->h[0] >> k) && lv->w[k] == max(1, lv->w[0] >> k), "%s: level %d is %d x %d, expected %d x %d", fn, k,
+                        lv->h[k], lv->w[k], max(1, lv->h[0] >> k), max(1, lv->w[0] >> k));
+        MCS_REQUIRE(lv->batch_stride[k] == (int64_t)lv->h[k] * lv->w[k] * lv->C || (lv->batch_stride[k] == 0 && Bt == 1),
+                    "%s: level %d batch_stride must be H*W*C (or 0 with Bt = 1)", fn, k);
+        MCS_REQUIRE(((uintptr_t)lv->ptr[k] & 3) == 0, "%s: level %d is not 4-byte aligned", fn, k);
+    }
+    MCS_REQUIRE(any, "%s: null pointer (no level given)", fn);
+    return 0;
+}
+
+MipFlat mip_flat(const mcs_texture_levels &lv, int32_t Bt, int64_t per)
+{
+    MipFlat f{};
+    int64_t e = 0;
+    for (int k = 0; k < lv.n_levels; ++k) f.end[k] = e += (lv.batch_stride[k] ? Bt : 1) * (int64_t)lv.h[k] * lv.w[k] * per;
+    return f;
+}
+
+unsigned flat_blocks(int64_t n) { return (unsigned)std::min<int64_t>((n + 255) / 256, 132 * 16); }
+
 }  // namespace
 
 extern "C" {
@@ -443,6 +651,53 @@ int mcs_texture_bwd(const mcs_texture_levels *tex, const float *uv, const float 
     a.uv = uv; a.uv_da = uv_da; a.dy = d_out; a.duv = d_uv; a.duv_da = mip ? d_uv_da : nullptr;
     a.B = B; a.H = H; a.W = W; a.mip = mip; a.clamp = boundary_mode == MCS_TEX_CLAMP; a.want_tex = any_tex;
     return tex_launch(a, (cudaStream_t)stream, true);
+}
+
+int32_t mcs_mip_chain_fwd_launches(int32_t n_levels) { return n_levels < 2 ? 0 : (n_levels - 1 + MIP_STEPS - 1) / MIP_STEPS; }
+
+int mcs_mip_chain_fwd(const mcs_texture_levels *chain, int32_t Bt, mcs_stream stream)
+{
+    if (int e = mip_validate("mcs_mip_chain_fwd", chain, Bt, 2, true, false)) return e;
+    const int L = chain->n_levels - 1;
+    for (int s = 0; s < L; s += MIP_STEPS) {
+        const dim3 grid((chain->w[s + 1] + 15) / 16, (chain->h[s + 1] + 15) / 16, Bt);
+        k_mip_down<<<grid, 256, 0, (cudaStream_t)stream>>>(*chain, s, min(MIP_STEPS, L - s));
+        MCS_LAUNCH_CHECK();
+    }
+    return 0;
+}
+
+int mcs_mip_chain_bwd(const mcs_texture_levels *grads, int32_t Bt, float *d_base, mcs_stream stream)
+{
+    if (int e = mip_validate("mcs_mip_chain_bwd", grads, Bt, 2, true, true)) return e;
+    MCS_REQUIRE(d_base != nullptr, "mcs_mip_chain_bwd: null pointer (d_base)");
+    MCS_REQUIRE(((uintptr_t)d_base & 3) == 0, "mcs_mip_chain_bwd: d_base is not 4-byte aligned");
+    int top = grads->n_levels - 1;
+    while (grads->ptr[top] == nullptr) --top;
+    const dim3 grid((grads->w[0] + FOLD_TILE - 1) / FOLD_TILE, (grads->h[0] + FOLD_TILE - 1) / FOLD_TILE, Bt);
+    k_mip_fold<<<grid, 256, 0, (cudaStream_t)stream>>>(*grads, top, d_base);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_mip_clamp(const mcs_texture_levels *levels, int32_t Bt, const float *lo, const float *hi, mcs_stream stream)
+{
+    if (int e = mip_validate("mcs_mip_clamp", levels, Bt, 1, false, false)) return e;
+    MCS_REQUIRE(lo != nullptr && hi != nullptr, "mcs_mip_clamp: null pointer (lo / hi)");
+    const MipFlat f = mip_flat(*levels, Bt, levels->C);
+    k_mip_clamp<<<flat_blocks(f.end[levels->n_levels - 1]), 256, 0, (cudaStream_t)stream>>>(*levels, f, levels->n_levels, lo, hi);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_mip_normalize(const mcs_texture_levels *levels, int32_t Bt, mcs_stream stream)
+{
+    if (int e = mip_validate("mcs_mip_normalize", levels, Bt, 1, false, false)) return e;
+    MCS_REQUIRE(levels->C == 3, "mcs_mip_normalize: C must be 3 (got %d)", levels->C);
+    const MipFlat f = mip_flat(*levels, Bt, 1);
+    k_mip_normalize<<<flat_blocks(f.end[levels->n_levels - 1]), 256, 0, (cudaStream_t)stream>>>(*levels, f, levels->n_levels);
+    MCS_LAUNCH_CHECK();
+    return 0;
 }
 
 }  // extern "C"

@@ -75,6 +75,9 @@ def build(force=False):
 # the tables against the sources).  REAL is a scalar `real`: c_float in the fp32 build, c_double in the fp64 one.
 REAL = "real"
 _P, _I, _I64 = C.c_void_p, C.c_int, C.c_int64
+# the `terms` mode of the entry points that scatter (test-only): the sum of the terms, the sum of their absolute values, or the number of
+# non-zero terms.  With n terms of absolute sum A, summing them in another order changes the sum by at most about 2 (n - 1) 2^-24 A.
+TERMS = {"sum": 0, "abs": 1, "count": 2}
 
 
 class CLib:

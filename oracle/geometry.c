@@ -5,9 +5,12 @@
  * G-buffer producer's geometry gradients and screen-space derivatives: the barycentrics of the clip-space triangle and their adjoint
  * (rasterize backward), the adjoint of interpolate with respect to rast, edge adjacency, pixel-pair analytic antialiasing, rast_db,
  * interpolate's attribute derivatives out_da, their adjoints (d attr, d rast_db, d rast_db -> d pos), and interpolate's forward in the
- * kernel's operation order.  No reference code exists for them (nvdiffrast is absent); the semantics are those stated in
- * nvdiffrecmc_b200/csrc/raster.cu.  Compile with -ffp-contract=off: the antialias pair decisions, rast_db, out_da and d rast_db are
- * evaluated in the same explicitly rounded operation order as the CUDA kernels.  Loaded by oracle/geometry.py.
+ * kernel's operation order.  Every entry point that scatters (d pos of rasterize, rast_db and antialias, d attr of interpolate and
+ * interpolate_da) takes a `terms` mode (test-only): 0 sums the per-pixel terms, 1 sums their absolute values, 2 counts the non-zero ones
+ * (the bound on the rounding of summing them in another order); the one-writer outputs are the same in every mode.  No reference code
+ * exists for them (nvdiffrast is absent); the semantics are those stated in nvdiffrecmc_b200/csrc/raster.cu.  Compile with
+ * -ffp-contract=off: the antialias pair decisions, rast_db, out_da and d rast_db are evaluated in the same explicitly rounded operation
+ * order as the CUDA kernels.  Loaded by oracle/geometry.py.
  */
 #include <math.h>
 #include <stdint.h>
@@ -28,6 +31,9 @@ typedef float real;
 typedef struct { real x, y, z; } v3;
 
 int geo_sizeof_real(void) { return (int)sizeof(real); }
+
+/* the term a scatter adds in mode `terms`: the term (0), its absolute value (1) or 1 when it is non-zero (2) */
+static inline real term_of(real t, int terms) { return terms == 0 ? t : (terms == 1 ? R_FABS(t) : (real)(t != RC(0))); }
 
 /* ================================================================================================================================
  * Geometry gradients of the G-buffer producer (nvdiffrecmc_b200/csrc/raster.cu states the semantics and the derivation):
@@ -70,7 +76,8 @@ void orc_raster_bary(int B, int H, int W, int64_t pos_bs, const real *pos, int T
     }
 }
 
-void orc_raster_bwd(int B, int H, int W, int64_t pos_bs, const real *pos, int T, const int32_t *tris, const real *rast, const real *d_rast, real *d_pos)
+void orc_raster_bwd(int B, int H, int W, int64_t pos_bs, const real *pos, int T, const int32_t *tris, const real *rast, const real *d_rast, real *d_pos,
+                    int terms)
 {
     for (int64_t i = 0; i < (int64_t)B * H * W; ++i) {
         const int ix = (int)(i % W), iy = (int)((i / W) % H), b = (int)(i / ((int64_t)W * H));
@@ -87,7 +94,7 @@ void orc_raster_bwd(int B, int H, int W, int64_t pos_bs, const real *pos, int T,
             const real dax = gs[k2] * ay[k1] - gs[k1] * ay[k2];
             const real day = gs[k1] * ax[k2] - gs[k2] * ax[k1];
             real *d = d_pos + b * pos_bs + 4 * (size_t)tri[k];
-            d[0] += dax; d[1] += day; d[3] += -px * dax - py * day;
+            d[0] += term_of(dax, terms); d[1] += term_of(day, terms); d[3] += term_of(-px * dax - py * day, terms);
         }
     }
 }
@@ -109,6 +116,25 @@ void orc_interpolate_bwd_rast(int B, int H, int W, int C, int64_t attr_bs, const
             }
         }
         d_rast[4 * i] = du; d_rast[4 * i + 1] = dv; d_rast[4 * i + 2] = 0; d_rast[4 * i + 3] = 0;
+    }
+}
+
+/* d attr (accumulated) of interpolate: vertex k of the pixel's triangle gets w_k g, with (w0, w1, w2) = (u, v, (1 - u) - v), in pixel,
+ * channel, vertex order (k_interpolate<1/2>'s terms) */
+void orc_interpolate_bwd_attr(int B, int H, int W, int C, int64_t attr_bs, int T, const int32_t *tris, const real *rast, const real *d_out,
+                              real *d_attr, int terms)
+{
+    for (int64_t i = 0; i < (int64_t)B * H * W; ++i) {
+        const int b = (int)(i / ((int64_t)W * H));
+        const int id = rast_tid(rast + 4 * i, T);
+        if (id < 0) continue;
+        real *D = d_attr + b * attr_bs;
+        const int32_t *tri = tris + 3 * (size_t)id;
+        const real w[3] = {rast[4 * i], rast[4 * i + 1], RC(1) - rast[4 * i] - rast[4 * i + 1]};
+        for (int c = 0; c < C; ++c) {
+            const real g = d_out[i * C + c];
+            for (int k = 0; k < 3; ++k) D[(size_t)tri[k] * C + c] += term_of(w[k] * g, terms);
+        }
     }
 }
 
@@ -270,11 +296,11 @@ void orc_antialias_fwd(int B, int H, int W, int C, const real *color, const real
     }
 }
 
-static void aa_edge_grad(const AAEdge *e, real px, real py, real s, real *dA, real *dB)
+static void aa_edge_grad(const AAEdge *e, real px, real py, real s, real *dA, real *dB, int terms)
 {
     const real ax = e->A.x - px * e->A.z, ay = e->A.y - py * e->A.z, bx = e->Bv.x - px * e->Bv.z, by = e->Bv.y - py * e->Bv.z;
-    dA[0] += s * by; dA[1] -= s * bx; dA[3] += s * (py * bx - px * by);
-    dB[0] -= s * ay; dB[1] += s * ax; dB[3] += s * (px * ay - py * ax);
+    dA[0] += term_of(s * by, terms); dA[1] += term_of(-(s * bx), terms); dA[3] += term_of(s * (py * bx - px * by), terms);
+    dB[0] += term_of(-(s * ay), terms); dB[1] += term_of(s * ax, terms); dB[3] += term_of(s * (px * ay - py * ax), terms);
 }
 
 /* d_color (overwritten) as the kernel gathers it: start from g_p and walk p's pairs in the order left, right, up, down; a pair p gains
@@ -304,9 +330,9 @@ void orc_antialias_bwd_color(int B, int H, int W, int C, const real *color, cons
 }
 
 /* backward, written as a scatter over the pairs: d_color (overwritten; orc_antialias_bwd_color gathers it in the kernel's order) and
- * d_pos (accumulated) */
+ * d_pos (accumulated in the `terms` mode: two terms per pair and element, the front and the other pixel's) */
 void orc_antialias_bwd(int B, int H, int W, int C, const real *color, const real *rast, int64_t pos_bs, const real *pos, int T, const int32_t *tris,
-                       const int32_t *adj, const real *d_out, real *d_color, real *d_pos)
+                       const int32_t *adj, const real *d_out, real *d_color, real *d_pos, int terms)
 {
     const OrcAA p = aa_make(B, H, W, C, color, rast, pos_bs, pos, T, tris, adj);
     memcpy(d_color, d_out, sizeof(real) * (size_t)B * H * W * C);
@@ -329,8 +355,8 @@ void orc_antialias_bwd(int B, int H, int W, int C, const real *color, const real
             if (gain == front) dLdt = -dLdt;               /* f gains (1/2 - t)(c_o - c_f); o gains (t - 1/2)(c_f - c_o) */
             const real D = e.ef - e.eo;
             real *dA = d_pos + b * pos_bs + 4 * (size_t)e.va, *dB = d_pos + b * pos_bs + 4 * (size_t)e.vb;
-            aa_edge_grad(&e, fx, fy, dLdt * (-e.eo / (D * D)), dA, dB);
-            aa_edge_grad(&e, ox, oy, dLdt * (e.ef / (D * D)), dA, dB);
+            aa_edge_grad(&e, fx, fy, dLdt * (-e.eo / (D * D)), dA, dB, terms);
+            aa_edge_grad(&e, ox, oy, dLdt * (e.ef / (D * D)), dA, dB, terms);
         }
     }
 }
@@ -401,7 +427,8 @@ void orc_rast_db(int B, int H, int W, int64_t pos_bs, const real *pos, int T, co
 }
 
 /* d rast_db -> d pos (accumulated): L = sum_{c = u, v; p = px, py} h_cp (ds_c/dp - c dS/dp) / S, h = d rast_db scaled by 2/W, 2/H */
-void orc_rast_db_bwd(int B, int H, int W, int64_t pos_bs, const real *pos, int T, const int32_t *tris, const real *rast, const real *d_db, real *d_pos)
+void orc_rast_db_bwd(int B, int H, int W, int64_t pos_bs, const real *pos, int T, const int32_t *tris, const real *rast, const real *d_db, real *d_pos,
+                     int terms)
 {
     const real sx = RC(2) / (real)W, sy = RC(2) / (real)H;
     for (int64_t i = 0; i < (int64_t)B * H * W; ++i) {
@@ -424,9 +451,9 @@ void orc_rast_db_bwd(int B, int H, int W, int64_t pos_bs, const real *pos, int T
             const real dax = gs[k2] * d.ay[k1] - gs[k1] * d.ay[k2];
             const real day = gs[k1] * d.ax[k2] - gs[k2] * d.ax[k1];
             real *o = d_pos + b * pos_bs + 4 * (size_t)tri[k];
-            o[0] += dax + ey[k1] * d.w[k2] - ey[k2] * d.w[k1];
-            o[1] += day + ex[k2] * d.w[k1] - ex[k1] * d.w[k2];
-            o[3] += -d.px * dax - d.py * day + ex[k1] * d.y[k2] - ex[k2] * d.y[k1] + ey[k2] * d.x[k1] - ey[k1] * d.x[k2];
+            o[0] += term_of(dax + ey[k1] * d.w[k2] - ey[k2] * d.w[k1], terms);
+            o[1] += term_of(day + ex[k2] * d.w[k1] - ex[k1] * d.w[k2], terms);
+            o[3] += term_of(-d.px * dax - d.py * day + ex[k1] * d.y[k2] - ex[k2] * d.y[k1] + ey[k2] * d.x[k1] - ey[k1] * d.x[k2], terms);
         }
     }
 }
@@ -452,9 +479,10 @@ void orc_interpolate_da(int B, int H, int W, int C, int64_t attr_bs, const real 
     }
 }
 
-/* d attr (accumulated) and d rast_db (overwritten) of out_da */
+/* d attr (accumulated in the `terms` mode) and d rast_db (overwritten) of out_da.  The third vertex's term is -(a0 + a1); its statistics
+ * are those of a0 and a1 (|a0| + |a1|, and 1 when either is non-zero), because the kernel forms it from the group sums of a0 and a1. */
 void orc_interpolate_da_bwd(int B, int H, int W, int C, int64_t attr_bs, const real *attr, int T, const int32_t *tris, const real *rast, const real *db,
-                            int n, const int32_t *idx, const real *d_out_da, real *d_attr, real *d_db)
+                            int n, const int32_t *idx, const real *d_out_da, real *d_attr, real *d_db, int terms)
 {
     for (int64_t i = 0; i < (int64_t)B * H * W; ++i) {
         const int b = (int)(i / ((int64_t)W * H));
@@ -469,7 +497,10 @@ void orc_interpolate_da_bwd(int B, int H, int W, int C, int64_t attr_bs, const r
                 const real gX = d_out_da[(i * n + k) * 2], gY = d_out_da[(i * n + k) * 2 + 1];
                 const real a2 = A[(size_t)tri[2] * C + c], d0 = A[(size_t)tri[0] * C + c] - a2, d1 = A[(size_t)tri[1] * C + c] - a2;
                 const real a0 = gX * g[0] + gY * g[1], a1 = gX * g[2] + gY * g[3];
-                D[(size_t)tri[0] * C + c] += a0; D[(size_t)tri[1] * C + c] += a1; D[(size_t)tri[2] * C + c] -= a0 + a1;
+                D[(size_t)tri[0] * C + c] += term_of(a0, terms); D[(size_t)tri[1] * C + c] += term_of(a1, terms);
+                if (terms == 0) D[(size_t)tri[2] * C + c] -= a0 + a1;
+                else if (terms == 1) D[(size_t)tri[2] * C + c] += R_FABS(a0) + R_FABS(a1);
+                else D[(size_t)tri[2] * C + c] += (real)(a0 != RC(0) || a1 != RC(0));
                 e[0] = e[0] + gX * d0; e[1] = e[1] + gY * d0; e[2] = e[2] + gX * d1; e[3] = e[3] + gY * d1;
             }
         }

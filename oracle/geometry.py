@@ -8,7 +8,7 @@ and the developer tools import it; ``nvdiffrecmc_b200`` never does.
 """
 import numpy as np
 
-from oracle import CLib, _I, _I64, _P
+from oracle import TERMS, CLib, _I, _I64, _P
 
 
 class GeometryOracle(CLib):
@@ -16,18 +16,19 @@ class GeometryOracle(CLib):
     SIGS = {
         "geo_sizeof_real": ([], _I),
         "orc_raster_bary": ([_I] * 3 + [_I64, _P, _I] + [_P] * 3, None),
-        "orc_raster_bwd": ([_I] * 3 + [_I64, _P, _I] + [_P] * 4, None),
+        "orc_raster_bwd": ([_I] * 3 + [_I64, _P, _I] + [_P] * 4 + [_I], None),
+        "orc_interpolate_bwd_attr": ([_I] * 4 + [_I64, _I] + [_P] * 4 + [_I], None),
         "orc_interpolate_bwd_rast": ([_I] * 4 + [_I64, _P, _I] + [_P] * 4, None),
         "orc_aa_topology": ([_I, _P, _P], None),
         "orc_antialias_pair_t": ([_I] * 3 + [_P, _I64, _P, _I] + [_P] * 3, None),
         "orc_antialias_fwd": ([_I] * 4 + [_P, _P, _I64, _P, _I] + [_P] * 3, None),
         "orc_antialias_bwd_color": ([_I] * 4 + [_P, _P, _I64, _P, _I] + [_P] * 4, None),
-        "orc_antialias_bwd": ([_I] * 4 + [_P, _P, _I64, _P, _I] + [_P] * 5, None),
+        "orc_antialias_bwd": ([_I] * 4 + [_P, _P, _I64, _P, _I] + [_P] * 5 + [_I], None),
         "orc_interpolate_fwd": ([_I] * 4 + [_I64, _P, _I] + [_P] * 3, None),
         "orc_rast_db": ([_I] * 3 + [_I64, _P, _I] + [_P] * 3, None),
-        "orc_rast_db_bwd": ([_I] * 3 + [_I64, _P, _I] + [_P] * 4, None),
+        "orc_rast_db_bwd": ([_I] * 3 + [_I64, _P, _I] + [_P] * 4 + [_I], None),
         "orc_interpolate_da": ([_I] * 4 + [_I64, _P, _I] + [_P] * 3 + [_I, _P, _P], None),
-        "orc_interpolate_da_bwd": ([_I] * 4 + [_I64, _P, _I] + [_P] * 3 + [_I] + [_P] * 4, None),
+        "orc_interpolate_da_bwd": ([_I] * 4 + [_I64, _P, _I] + [_P] * 3 + [_I] + [_P] * 4 + [_I], None),
     }
 
     def _geo(self, pos, rast, tris):
@@ -49,11 +50,24 @@ class GeometryOracle(CLib):
         self.lib.orc_raster_bary(B, H, W, pbs, pos.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, uv.ctypes.data)
         return uv
 
-    def raster_bwd(self, pos, tris, rast, d_rast):
-        """d pos (shape of pos) from d rast[...,0:2] through the barycentrics of pos."""
+    def raster_bwd(self, pos, tris, rast, d_rast, terms="sum"):
+        """d pos (shape of pos) from d rast[...,0:2] through the barycentrics of pos.  terms: the sum of the per-pixel terms, the sum of
+        their absolute values ("abs") or the number of non-zero terms ("count"), as for every scatter below."""
         pos, rast, tris, B, H, W, pbs = self._geo(pos, rast, tris)
         g = self._a(d_rast); d = np.zeros_like(pos)
-        self.lib.orc_raster_bwd(B, H, W, pbs, pos.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, g.ctypes.data, d.ctypes.data)
+        self.lib.orc_raster_bwd(B, H, W, pbs, pos.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, g.ctypes.data, d.ctypes.data,
+                                TERMS[terms])
+        return d
+
+    def interpolate_bwd_attr(self, attr_shape, tris, rast, d_out, terms="sum"):
+        """d attr (shape attr_shape: [V,C] or [B,V,C]) of interpolate: vertex k of the pixel's triangle gets w_k g, (w0, w1, w2) = (u, v,
+        (1 - u) - v), summed in pixel, channel, vertex order."""
+        rast = self._a(rast); tris = np.ascontiguousarray(tris, np.int32)
+        B, H, W = rast.shape[:3]
+        Cn = attr_shape[-1]
+        g = self._a(d_out, (B, H, W, Cn)); d = np.zeros(attr_shape, self.dt)
+        self.lib.orc_interpolate_bwd_attr(B, H, W, Cn, attr_shape[-2] * Cn if len(attr_shape) == 3 else 0, tris.shape[0], tris.ctypes.data,
+                                          rast.ctypes.data, g.ctypes.data, d.ctypes.data, TERMS[terms])
         return d
 
     def interpolate_bwd_rast(self, attr, tris, rast, d_out):
@@ -87,13 +101,13 @@ class GeometryOracle(CLib):
         self.lib.orc_antialias_fwd(*args, out.ctypes.data)
         return out
 
-    def antialias_bwd(self, color, rast, pos, tris, d_out, adj=None, scatter=False):
+    def antialias_bwd(self, color, rast, pos, tris, d_out, adj=None, scatter=False, terms="sum"):
         """-> (d_color, d_pos).  d_color is gathered per pixel in the kernel's order (the fp32 build equals k_antialias<true> bit for
-        bit), or with scatter=True accumulated pair by pair; d_pos is always the pair-by-pair scatter."""
+        bit), or with scatter=True accumulated pair by pair; d_pos is always the pair-by-pair scatter, in the `terms` mode."""
         keep, args = self._aa_args(color, rast, pos, tris, adj)
         g = self._a(d_out, keep[0].shape)
         dc = np.zeros_like(keep[0]); dp = np.zeros_like(keep[2])
-        self.lib.orc_antialias_bwd(*args, g.ctypes.data, dc.ctypes.data, dp.ctypes.data)
+        self.lib.orc_antialias_bwd(*args, g.ctypes.data, dc.ctypes.data, dp.ctypes.data, TERMS[terms])
         if not scatter:
             self.lib.orc_antialias_bwd_color(*args, g.ctypes.data, dc.ctypes.data)
         return dc, dp
@@ -121,11 +135,12 @@ class GeometryOracle(CLib):
         self.lib.orc_rast_db(B, H, W, pbs, pos.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, db.ctypes.data)
         return db
 
-    def rast_db_bwd(self, pos, tris, rast, d_db):
-        """d pos (shape of pos) from d rast_db."""
+    def rast_db_bwd(self, pos, tris, rast, d_db, terms="sum"):
+        """d pos (shape of pos) from d rast_db, in the `terms` mode."""
         pos, rast, tris, B, H, W, pbs = self._geo(pos, rast, tris)
         g = self._a(d_db); d = np.zeros_like(pos)
-        self.lib.orc_rast_db_bwd(B, H, W, pbs, pos.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, g.ctypes.data, d.ctypes.data)
+        self.lib.orc_rast_db_bwd(B, H, W, pbs, pos.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, g.ctypes.data, d.ctypes.data,
+                                 TERMS[terms])
         return d
 
     @staticmethod
@@ -146,14 +161,15 @@ class GeometryOracle(CLib):
                                     out.ctypes.data)
         return out
 
-    def interpolate_da_bwd(self, attr, tris, rast, db, d_out_da, diff_attrs="all"):
-        """-> (d attr, d rast_db) of out_da."""
+    def interpolate_da_bwd(self, attr, tris, rast, db, d_out_da, diff_attrs="all", terms="sum"):
+        """-> (d attr, d rast_db) of out_da; d attr in the `terms` mode, where the third vertex's term -(a0 + a1) counts as |a0| + |a1|
+        and as one term when a0 or a1 is non-zero."""
         attr, rast, tris, B, H, W, Cn, abs_ = self._attr(attr, tris, rast)
         db = self._a(db); g = self._a(d_out_da)
         n, keep, ip = self._sel(diff_attrs, Cn)
         da = np.zeros_like(attr); ddb = np.zeros((B, H, W, 4), self.dt)
         self.lib.orc_interpolate_da_bwd(B, H, W, Cn, abs_, attr.ctypes.data, tris.shape[0], tris.ctypes.data, rast.ctypes.data, db.ctypes.data, n,
-                                        ip, g.ctypes.data, da.ctypes.data, ddb.ctypes.data)
+                                        ip, g.ctypes.data, da.ctypes.data, ddb.ctypes.data, TERMS[terms])
         return da, ddb
 
 

@@ -2,7 +2,8 @@
  *
  * A plain-C restatement of the contract in nvdiffrecmc_b200/csrc/hashgrid.cu, written independently of the kernels:
  *   level table (double precision), forward, d x (levels ascending, corners ascending) and d params (a sequential scatter in point,
- *   level, corner order).
+ *   level, corner order).  d params takes a `terms` mode (test-only): 0 sums the terms w_c g, 1 sums their absolute values, 2 counts the
+ *   non-zero ones; d x is the same in every mode.
  * Two builds of this file (oracle/hashgrid.py): fp32 (`real` = float, compared bit for bit with the CUDA forward and d x) and fp64
  * (-DORACLE_F64, checked by finite differences and the adjoint identity).  Compile with -ffp-contract=off: every product and sum is one
  * IEEE round-to-nearest operation, the fma of p_d is the only fused one.
@@ -94,6 +95,9 @@ static void corner_weights(const cell_t *cl, int c, real w1[3])
     for (int d = 0; d < 3; ++d) w1[d] = ((c >> d) & 1) ? cl->t[d] : (real)1 - cl->t[d];
 }
 
+/* dst + term (terms 0), + |term| (1) or + (term != 0) (2): the scatter's term statistics */
+static real hg_term(real t, int terms) { return terms == 0 ? t : (terms == 1 ? (real)fabs((double)t) : (real)(t != 0)); }
+
 /* x [n,3]; params [2 * offset[L]]; out [n, 2L] */
 void hg_fwd(const real *x, int64_t n, const real *params, int L, const uint64_t *offset, const uint32_t *res, const float *scale,
             uint32_t dense_mask, real *out)
@@ -118,9 +122,9 @@ void hg_fwd(const real *x, int64_t n, const real *params, int L, const uint64_t 
     }
 }
 
-/* d_out [n, 2L]; d_params (may be null) accumulates; d_x (may be null) is overwritten. */
+/* d_out [n, 2L]; d_params (may be null) accumulates in the `terms` mode; d_x (may be null) is overwritten. */
 void hg_bwd(const real *x, int64_t n, const real *params, int L, const uint64_t *offset, const uint32_t *res, const float *scale,
-            uint32_t dense_mask, const real *d_out, real *d_params, real *d_x)
+            uint32_t dense_mask, const real *d_out, real *d_params, real *d_x, int terms)
 {
     if (d_x) {
 #pragma omp parallel for schedule(static)
@@ -157,8 +161,8 @@ void hg_bwd(const real *x, int64_t n, const real *params, int L, const uint64_t 
                     corner_weights(&cl, c, w1);
                     const real w = (w1[0] * w1[1]) * w1[2];
                     real *dp = d_params + 2 * (offset[l] + corner_index(&cl, c, (dense_mask >> l) & 1u, res[l], size));
-                    dp[0] = dp[0] + w * g0;
-                    dp[1] = dp[1] + w * g1;
+                    dp[0] = dp[0] + hg_term(w * g0, terms);
+                    dp[1] = dp[1] + hg_term(w * g1, terms);
                 }
             }
         }

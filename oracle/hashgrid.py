@@ -9,7 +9,7 @@ import ctypes as C
 
 import numpy as np
 
-from oracle import CLib, _I, _I64, _P
+from oracle import TERMS, CLib, _I, _I64, _P
 
 # the configuration render/mlptexture.py:57-70 hard-codes
 REF_CONFIG = {"otype": "HashGrid", "n_levels": 16, "n_features_per_level": 2, "log2_hashmap_size": 19, "base_resolution": 16,
@@ -29,7 +29,7 @@ class HashGridOracle(CLib):
         "hg_sizeof_real": ([], _I),
         "hg_levels": ([_I, _I, C.c_double, C.c_double] + [_P] * 4, _I),
         "hg_fwd": ([_P, _I64, _P, _I, _P, _P, _P, C.c_uint32, _P], None),
-        "hg_bwd": ([_P, _I64, _P, _I, _P, _P, _P, C.c_uint32] + [_P] * 3, None),
+        "hg_bwd": ([_P, _I64, _P, _I, _P, _P, _P, C.c_uint32] + [_P] * 3 + [_I], None),
     }
 
     def levels(self, cfg):
@@ -57,15 +57,16 @@ class HashGridOracle(CLib):
         self.lib.hg_fwd(x.ctypes.data, x.shape[0], p.ctypes.data, *a, out.ctypes.data)
         return out
 
-    def backward(self, x, params, lv, d_out, want_params=True, want_x=True):
-        """-> (d_params or None, d_x or None)"""
+    def backward(self, x, params, lv, d_out, want_params=True, want_x=True, terms="sum"):
+        """-> (d_params or None, d_x or None).  terms: d params as the sum of its terms w_c g, the sum of their absolute values ("abs") or
+        the number of non-zero terms ("count")."""
         x = self._a(x).reshape(-1, 3); p = self._a(params); g = self._a(d_out)
         assert g.shape == (x.shape[0], 2 * lv["n_levels"])
         dp = np.zeros_like(p) if want_params else None
         dx = np.zeros_like(x) if want_x else None
         keep, a = self._args(lv)
         self.lib.hg_bwd(x.ctypes.data, x.shape[0], p.ctypes.data, *a, g.ctypes.data, dp.ctypes.data if want_params else None,
-                        dx.ctypes.data if want_x else None)
+                        dx.ctypes.data if want_x else None, TERMS[terms])
         return dp, dx
 
 

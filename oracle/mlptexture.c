@@ -98,10 +98,11 @@ void mlt_fwd(const real *t, int64_t n, const real *aabb, const real *min_max, co
     free(xn); free(xc); free(e);
 }
 
-/* d_out [n,C]; d_params (may be null) accumulates; d_t [n,3] and d_w [hidden * 1024 + 32 C] (each may be null) are overwritten. */
+/* d_out [n,C]; d_params (may be null) accumulates in hg_bwd's `terms` mode; d_t [n,3] and d_w [hidden * 1024 + 32 C] (each may be null)
+ * are overwritten and the same in every mode. */
 void mlt_bwd(const real *t, int64_t n, const real *aabb, const real *min_max, const real *params, int L, const uint64_t *offset,
                    const uint32_t *res, const float *scale, uint32_t dense_mask, int hidden, int C, const real *w, const real *d_out,
-                   real *d_params, real *d_t, real *d_w)
+                   real *d_params, real *d_t, real *d_w, int terms)
 {
     const int nA = (hidden + 1) * 32, nD = hidden * 32 + C, nW = hidden * 1024 + C * 32;
     real *xn = malloc(sizeof(real) * 3 * (size_t)n + 1), *xc = malloc(sizeof(real) * 3 * (size_t)n + 1);
@@ -148,7 +149,7 @@ void mlt_bwd(const real *t, int64_t n, const real *aabb, const real *min_max, co
     }
     if (d_params || d_t) {
         real *dxc = d_t ? malloc(sizeof(real) * 3 * (size_t)n + 1) : NULL;
-        hg_bwd(xc, n, params, L, offset, res, scale, dense_mask, de, d_params, dxc);
+        hg_bwd(xc, n, params, L, offset, res, scale, dense_mask, de, d_params, dxc, terms);
         if (d_t) {
             for (int64_t i = 0; i < 3 * n; ++i) {
                 const int d = (int)(i % 3);

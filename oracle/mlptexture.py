@@ -11,7 +11,7 @@ import os
 
 import numpy as np
 
-from oracle import _HERE, _I, _I64, _P, LIBS
+from oracle import _HERE, _I, _I64, _P, LIBS, TERMS
 from oracle.hashgrid import HashGridOracle
 
 SOURCES = [os.path.join(_HERE, s) for s in LIBS["mlptexture"]]      # paths of the library's source and the hashgrid.c it includes
@@ -23,7 +23,7 @@ class MlpTextureOracle(HashGridOracle):
     SIGS = dict(HashGridOracle.SIGS, **{
         "mlt_exp": ([_P, _I64, _P], None),
         "mlt_fwd": ([_P, _I64] + [_P] * 3 + [_I, _P, _P, _P, C.c_uint32, _I, _I] + [_P] * 3, None),
-        "mlt_bwd": ([_P, _I64] + [_P] * 3 + [_I, _P, _P, _P, C.c_uint32, _I, _I] + [_P] * 5, None),
+        "mlt_bwd": ([_P, _I64] + [_P] * 3 + [_I, _P, _P, _P, C.c_uint32, _I, _I] + [_P] * 5 + [_I], None),
     })
 
     def exp(self, x):
@@ -50,8 +50,9 @@ class MlpTextureOracle(HashGridOracle):
         self.lib.mlt_fwd(*a, out.ctypes.data, enc.ctypes.data)
         return out, enc
 
-    def mlptex_backward(self, t, aabb, min_max, params, lv, weights, d_out, want_params=True, want_t=True, want_w=True):
-        """-> (d params or None, d t or None, [d W per layer] or None): the true gradients (no x128 on d params)."""
+    def mlptex_backward(self, t, aabb, min_max, params, lv, weights, d_out, want_params=True, want_t=True, want_w=True, terms="sum"):
+        """-> (d params or None, d t or None, [d W per layer] or None): the true gradients (no x128 on d params).  terms: d params in
+        hg_bwd's mode ("sum", "abs" or "count")."""
         keep, a = self._mlp_args(t, aabb, min_max, params, lv, weights)
         n, C, p = keep[0].shape[0], keep[2].shape[1], keep[3]
         g = self._a(d_out).reshape(n, C)
@@ -59,7 +60,7 @@ class MlpTextureOracle(HashGridOracle):
         dt = np.zeros((n, 3), self.dt) if want_t else None
         dw = np.zeros(keep[4].size, self.dt) if want_w else None
         self.lib.mlt_bwd(*a, g.ctypes.data, dp.ctypes.data if want_params else None, dt.ctypes.data if want_t else None,
-                               dw.ctypes.data if want_w else None)
+                               dw.ctypes.data if want_w else None, TERMS[terms])
         if want_w:
             sizes = [np.asarray(x).size for x in weights]
             dw = [d.reshape(np.asarray(x).shape) for d, x in zip(np.split(dw, np.cumsum(sizes)[:-1]), weights)]

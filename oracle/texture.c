@@ -5,6 +5,8 @@
  *   level of detail from the major axis of the pixel footprint, lam = 0.5 * log2(M) clamped to [0, L], trilinear blend of levels
  *   floor(lam) and floor(lam) + 1 (level l1 not read when the blend fraction is 0), and the three adjoints:
  *   d tex (a sequential scatter in pixel, channel-group, level, tap order), d uv and d uv_da (one writer per pixel).
+ * d tex takes a `terms` mode (test-only): 0 sums the terms (w_lvl w_ij) g_c, 1 sums their absolute values, 2 counts the non-zero ones;
+ * the one-writer outputs are the same in every mode.
  * Two builds of this file (oracle/texture.py): fp32 (`real` = float; log2 is the fixed algorithm of the contract, so the forward, d uv and
  * d uv_da equal the kernels' bit for bit) and fp64 (-DORACLE_F64, libm log2; checked by finite differences and the adjoint identity).
  * Compile with -ffp-contract=off: every product and sum is one IEEE round-to-nearest operation, in the order the contract writes it.
@@ -92,6 +94,9 @@ typedef struct {
     real fx, fy;
 } taps_t;
 
+/* dst + term (terms 0), + |term| (1) or + (term != 0) (2): the scatter's term statistics */
+static real term_of(real t, int terms) { return terms == 0 ? t : (terms == 1 ? (real)fabs((double)t) : (real)(t != 0)); }
+
 static taps_t taps(int C, int h, int w, int64_t bstride, int b, real u, real v, int clamp)
 {
     taps_t t;
@@ -161,7 +166,7 @@ void tex_fwd(int n_levels, int C, const real *const *ptr, const int *h, const in
 
 /* d_tex: n_levels pointers (null entries skipped) accumulated; d_uv [B,H,W,2], d_uv_da [B,H,W,4] overwritten (each may be null). */
 void tex_bwd(int n_levels, int C, const real *const *ptr, const int *h, const int *w, const int64_t *bstride, const real *uv, const real *uv_da,
-             int B, int H, int W, int mip, int clamp, const real *d_out, real *const *d_tex, real *d_uv, real *d_uv_da)
+             int B, int H, int W, int mip, int clamp, const real *d_out, real *const *d_tex, real *d_uv, real *d_uv_da, int terms)
 {
     const int64_t n = (int64_t)B * H * W;
     const int L = mip ? n_levels - 1 : 0;
@@ -199,7 +204,7 @@ void tex_bwd(int n_levels, int C, const real *const *ptr, const int *h, const in
                 const real wt[4] = {wl[s] * (oy * ox), wl[s] * (oy * t[s].fx), wl[s] * (t[s].fy * ox), wl[s] * (t[s].fy * t[s].fx)};
                 for (int c = 0; c < C; ++c) {
                     if (g[c] == 0) continue;
-                    for (int j = 0; j < 4; ++j) dt[t[s].o[j] + c] = dt[t[s].o[j] + c] + wt[j] * g[c];
+                    for (int j = 0; j < 4; ++j) dt[t[s].o[j] + c] = dt[t[s].o[j] + c] + term_of(wt[j] * g[c], terms);
                 }
             }
         }

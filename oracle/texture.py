@@ -9,7 +9,7 @@ import ctypes as C
 
 import numpy as np
 
-from oracle import CLib, _I, _P
+from oracle import TERMS, CLib, _I, _P
 
 FILTERS = {"linear": 0, "linear-mipmap-linear": 1}
 BOUNDARIES = {"wrap": 0, "clamp": 1}
@@ -26,7 +26,7 @@ class TextureOracle(CLib):
         "tex_sizeof_real": ([], _I),
         "tex_log2f": ([C.c_float], C.c_float),
         "tex_fwd": ([_I, _I] + [_P] * 6 + [_I] * 5 + [_P], None),
-        "tex_bwd": ([_I, _I] + [_P] * 6 + [_I] * 5 + [_P] * 4, None),
+        "tex_bwd": ([_I, _I] + [_P] * 6 + [_I] * 5 + [_P] * 4 + [_I], None),
     }
 
     def log2(self, x):
@@ -59,8 +59,10 @@ class TextureOracle(CLib):
         self.lib.tex_fwd(*a, uv.ctypes.data, da.ctypes.data if da is not None else None, B, H, W, mip, BOUNDARIES[boundary_mode], out.ctypes.data)
         return out
 
-    def backward(self, levels, uv, uv_da, d_out, filter_mode="linear", boundary_mode="wrap", want_tex=True, want_uv=True, want_uv_da=True):
-        """-> (list of d level or None, d uv or None, d uv_da or None); 'linear' returns one d level and no d uv_da."""
+    def backward(self, levels, uv, uv_da, d_out, filter_mode="linear", boundary_mode="wrap", want_tex=True, want_uv=True, want_uv_da=True,
+                 terms="sum"):
+        """-> (list of d level or None, d uv or None, d uv_da or None); 'linear' returns one d level and no d uv_da.  terms: d tex as the
+        sum of its terms (w_lvl w_ij) g_c, the sum of their absolute values ("abs") or the number of non-zero terms ("count")."""
         if FILTERS[filter_mode] == 0:
             levels = levels[:1]
         keep, a = self._levels(levels)
@@ -73,7 +75,8 @@ class TextureOracle(CLib):
         duv = np.zeros_like(uv) if want_uv else None
         dda = np.zeros((B, H, W, 4), self.dt) if (want_uv_da and mip) else None
         ptr = lambda x: x.ctypes.data if x is not None else None
-        self.lib.tex_bwd(*a, uv.ctypes.data, ptr(da), B, H, W, mip, BOUNDARIES[boundary_mode], g.ctypes.data, dtp, ptr(duv), ptr(dda))
+        self.lib.tex_bwd(*a, uv.ctypes.data, ptr(da), B, H, W, mip, BOUNDARIES[boundary_mode], g.ctypes.data, dtp, ptr(duv), ptr(dda),
+                         TERMS[terms])
         return dt, duv, dda
 
 

@@ -220,6 +220,98 @@ def check_per_element(op, got, f64, f32, ins, K, names, seed=0, exempt=None, flo
     return worst
 
 
+# ------------------------------------------------------------------------------------------ per-element bars of the float-atomic scatters
+U32 = 2.0 ** -24            # the unit roundoff of fp32
+
+
+def _gamma(k):
+    """gamma(k) = k u / (1 - k u), the relative bound of k fp32 roundings"""
+    k = np.asarray(k, np.float64) * U32
+    return k / (1.0 - k)
+
+
+def check_scatter_fp32(op, got, r32, a32, n32, tag="scatter"):
+    """A scatter whose terms the kernel computes bit for bit as the fp32 oracle does (d tex, hash-grid and MLP-texture d params,
+    texel_fetch d tex): the two add the same n fp32 terms in different orders, so with r32 / a32 / n32 the fp32 oracle's sum, sum of
+    absolute values and count of non-zero terms (terms="sum" / "abs" / "count"), every element must satisfy
+        |got - r32| <= 2 gamma(n - 1) a32 (1 + gamma(n)),
+    the deterministic bound of two summation orders (the factor covers the rounding of a32 itself).  Elements with n <= 2 are therefore
+    bit-identical (fp addition is commutative) and checked as such; the zero pattern and NaN / +-inf must be the fp32 oracle's.  Prints and
+    returns (worst |got - r32| / bound, largest n)."""
+    got, r, a, n = (np.asarray(x, np.float64) for x in (got, r32, a32, n32))
+    assert got.shape == r.shape == a.shape == n.shape, (op, got.shape, r.shape, a.shape, n.shape)
+    for pred, what in ((np.isnan, "NaN"), (np.isposinf, "+inf"), (np.isneginf, "-inf")):
+        bad = pred(got) != pred(r)
+        assert not bad.any(), "%s: %s at %d elements where the fp32 oracle disagrees (first %s)" % (
+            op, what, int(bad.sum()), tuple(np.argwhere(bad)[0]))
+    fin = np.isfinite(r) & np.isfinite(a)
+    zero = (got == 0) != (r == 0)
+    assert not (zero & fin).any(), "%s: zero pattern differs from the fp32 oracle's at %d elements (first %s: got %r, fp32 oracle %r, " \
+        "n %d)" % (op, int((zero & fin).sum()), tuple(np.argwhere(zero & fin)[0]), got[zero & fin][0], r[zero & fin][0], n[zero & fin][0])
+    few = fin & (n <= 2) & (got != r)
+    assert not few.any(), "%s: %d elements of at most two terms differ from the fp32 oracle (first %s: got %r, fp32 oracle %r, n %d)" % (
+        op, int(few.sum()), tuple(np.argwhere(few)[0]), got[few][0], r[few][0], n[few][0])
+    bound = 2.0 * _gamma(np.maximum(n - 1, 0)) * a * (1.0 + _gamma(n))
+    err = np.abs(got - r)
+    bad = fin & ~(err <= bound)
+    ratio = np.where(fin, np.divide(err, bound, out=np.where(err > 0, np.inf, 0.0), where=bound > 0), 0.0)
+    worst = float(ratio.max()) if ratio.size else 0.0
+    nmax = int(n[fin].max()) if fin.any() else 0
+    if bad.any():
+        ex = "; ".join("%s got %.9g r32 %.9g abs %.3g n %d bound %.3g" % (tuple(i), got[tuple(i)], r[tuple(i)], a[tuple(i)], n[tuple(i)],
+                                                                            bound[tuple(i)]) for i in np.argwhere(bad)[:3])
+        raise AssertionError("%s: %d of %d elements beyond 2 gamma(n-1) A (1 + gamma(n)) of the fp32 oracle (worst ratio %.3g): %s" % (
+            op, int(bad.sum()), int(fin.sum()), worst, ex))
+    print("[%s] %-60s worst ratio %.3g, largest n %d, over %d elements (%d of 1 or 2 terms, bit for bit)" % (
+        tag, op, worst, nmax, int(fin.sum()), int((fin & (n > 0) & (n <= 2)).sum())))
+    return worst, nmax
+
+
+def texel_fetch_stats(T, idx, g):
+    """texel_fetch's d tex [T,C] as the fp32 sum, abs sum and count of its terms g[i] (every i with 0 <= idx[i] < T), each a sequential
+    scatter in i order (np.add.at is unbuffered)"""
+    idx = np.asarray(idx).reshape(-1)
+    g = np.asarray(g, np.float32).reshape(idx.size, -1)
+    ok = (idx >= 0) & (idx < T)
+    out = []
+    for t in (g, np.abs(g), (g != 0).astype(np.float32)):
+        d = np.zeros((T, g.shape[1]), np.float32)
+        np.add.at(d, idx[ok], t[ok])
+        out.append(d)
+    return out
+
+
+def scatter_floor(n64, a64):
+    """The reduction floor of a scatter whose terms the kernel computes in its own order: n 2^-24 A with the fp64 oracle's count n and
+    absolute sum A (terms="count" / "abs"): the most that adding the same n terms in another fp32 order can change the sum."""
+    return np.asarray(n64, np.float64) * U32 * np.asarray(a64, np.float64)
+
+
+def check_scatter_fp64(op, got, f64, f32, ins, stats, K=16, seed=0, tag="scatter"):
+    """A scatter whose terms the kernel computes in its own order (rasterize / rast_db / antialias d pos, interpolate and
+    interpolate_da d attr): check_per_element against the fp64 oracle, every element, with a reduction floor.
+      f64(ins) / f32(ins): [the sum] of the fp64 / fp32 oracle;
+      ins: the inputs the sensitivity Delta perturbs (pos or rast_db, and the upstream gradient; rast stays fixed);
+      stats(f64): (count, abs) of the fp32 or fp64 oracle.
+    The floor is scatter_floor(max(n32, n64), max(A32, A64)).  Where the two oracles count a different number of terms (an antialias
+    pair or an e = 0 crossing decided differently, or a term exactly 0 in fp32 and tiny in fp64), the larger statistics bound the
+    rounding of either precision's terms, and |r32 - r64| in check_per_element's scale covers the term one of them lacks; those
+    elements are checked like the rest and counted in the printed line.  Rows (vertices) where the fp32 oracle has no term must be
+    exactly 0.  Prints and returns (worst ratio, largest n, elements whose counts differ)."""
+    got = np.asarray(got)
+    n32, a32 = (np.asarray(x, np.float64) for x in stats(False))
+    n64, a64 = (np.asarray(x, np.float64) for x in stats(True))
+    differ = n32 != n64
+    zero = (n32 == 0).all(-1)
+    assert (got[zero] == 0).all(), "%s: %d rows are nonzero where the fp32 oracle has no term" % (op, int((got[zero] != 0).any(-1).sum()))
+    floor = scatter_floor(np.maximum(n32, n64), np.maximum(a32, a64))
+    worst = check_per_element(op, [got], f64, f32, ins, K, ["per element"], seed=seed, floor=[floor], tag=tag)
+    nmax = int(np.maximum(n32, n64).max()) if n64.size else 0
+    print("[%s] %-60s largest n %d; fp32 and fp64 count differently at %d elements (checked with the larger statistics)" % (
+        tag, op, nmax, int(differ.sum())))
+    return worst, nmax, int(differ.sum())
+
+
 def _sample_px(B, H, W, n_rand=20000, seed=0, group=4):
     """Flat [B*H*W] pixel indices: rows 0, 1 and H-1 of views 0 and B-1, n_rand random pixels, and the last (ragged) `group`-pixel group."""
     n = B * H * W

@@ -1,18 +1,18 @@
 """GPU: the stage that gives the geometry its gradient, against the oracle (oracle/geometry.c) on the inputs where it can go wrong.
 antialias forward and d color, and interpolate forward and d rast, have one writer per output and equal the fp32 oracle bit for bit;
-antialias d pos, rasterize d pos (with and without rast_db) and interpolate d attr are float-atomic sums, held to the fp64 oracle run on
-the same fp32 inputs.  Every case starts from (v, f, mtx): rast comes from the GPU rasterize (bit-identical to the oracle's), pos from
-the oracle's xfm.  Cases: image shapes from 1x1 to 129x257 with B in {1, 3, 8}; every test camera (w <= 0 vertices, empty images);
-duplicated (non-manifold edges, z ties), zero-area, single-triangle, beyond-the-far-plane and holed meshes; grids whose edges run through
-pixel centres or midway between them (t = 1/2); every peel layer; ids >= T; one [V,4] shared by the batch; C from 1 to 12 with NaN and
-+-inf colours; the training shape."""
+antialias d pos, rasterize d pos (with and without rast_db) and interpolate d attr are float-atomic sums, held per element to the fp64
+oracle run on the same fp32 inputs, with the reduction floor n 2^-24 A of their terms (tests/common.py: check_scatter_fp64).  Every case
+starts from (v, f, mtx): rast comes from the GPU rasterize (bit-identical to the oracle's), pos from the oracle's xfm.  Cases: image shapes
+from 1x1 to 129x257 with B in {1, 3, 8}; every test camera (w <= 0 vertices, empty images); duplicated (non-manifold edges, z ties),
+zero-area, single-triangle, beyond-the-far-plane and holed meshes; grids whose edges run through pixel centres or midway between them
+(t = 1/2); every peel layer; ids >= T; one [V,4] shared by the batch; C from 1 to 12 with NaN and +-inf colours; the training shape."""
 import time
 
 import numpy as np
 import pytest
 import torch
 
-from common import RASTER_CAMERAS, nan_bits, oracle, pixel_grid_mesh, raster_mesh, raster_mtx, rel_l2, same_bits
+from common import RASTER_CAMERAS, check_scatter_fp64, nan_bits, oracle, pixel_grid_mesh, raster_mesh, raster_mtx, same_bits
 from oracle.geometry import geometry_oracle
 from nvdiffrecmc_b200 import synth
 
@@ -41,15 +41,15 @@ def _layer(ctx, m, res, k, pos=None, tri=None, grad_db=False):
     return out if grad_db else out[0]
 
 
-def _fp64_bar(got, ref32, ref64, what):
-    """rel-L2 from the fp64 oracle (run on the same fp32 inputs) within max(1e-5, 2 x the fp32 oracle's own distance from it), and
-    every row (vertex) the fp32 oracle leaves exactly 0 exactly 0.  The fp32 oracle makes the kernels' discrete decisions; the fp64
-    one can decide a pair or an e = 0 crossing differently (the on-centre grid, collapsed triangles), so its zero rows can differ."""
-    bar = max(1e-5, 2 * rel_l2(ref32, ref64))
-    err = rel_l2(got, ref64)
-    assert err <= bar, "%s: rel-L2 %.3e from the fp64 oracle, bar %.3e" % (what, err, bar)
-    zero = (ref32 == 0).all(-1)
-    assert (got[zero] == 0).all(), "%s: %d rows are nonzero where the fp32 oracle's are 0" % (what, (got[zero] != 0).any(-1).sum())
+def _geo(f64):
+    return geometry_oracle(f64=f64)
+
+
+def _bar(what, got, fn, ins, seed=0):
+    """check_scatter_fp64 of one scatter: fn(o, ins, terms) is the oracle o's output on the inputs ins (pos or rast_db, and the
+    upstream gradients, which Delta perturbs) in the mode `terms`"""
+    return check_scatter_fp64(what, got, lambda x: [fn(_geo(True), x, "sum")], lambda x: [fn(_geo(False), x, "sum")], ins,
+                              lambda f64: (fn(_geo(f64), ins, "count"), fn(_geo(f64), ins, "abs")), seed=seed, tag="geometry")
 
 
 def _poison(color, rast):
@@ -63,7 +63,7 @@ def _poison(color, rast):
 
 def _check_antialias(dev, f, pos, rast, C, seed, poison=False):
     """antialias_topology equal to the oracle's; forward and d color bit for bit (d color the same with and without pos requiring grad);
-    d pos at the fp64 bar, exactly 0 on vertices with w <= 0, and the same without color requiring grad."""
+    d pos per element against the fp64 oracle, exactly 0 on vertices with w <= 0, and the same without color requiring grad."""
     from nvdiffrecmc_b200.raster import antialias, antialias_topology
     g32, g64 = geometry_oracle(), geometry_oracle(f64=True)
     rng = np.random.default_rng(seed)
@@ -82,8 +82,8 @@ def _check_antialias(dev, f, pos, rast, C, seed, poison=False):
     dc32, dp32 = g32.antialias_bwd(color, rast, pos, f, g, adj)
     dc, dp = col.grad.cpu().numpy(), p.grad.cpu().numpy()
     assert same_bits(dc, dc32), "antialias d color: %d of %d values differ" % ((dc != dc32).sum(), dc.size)
-    _, dp64 = g64.antialias_bwd(color, rast, pos, f, g, adj)
-    _fp64_bar(dp, dp32, dp64, "antialias d pos")
+    _, dp64 = g64.antialias_bwd(color, rast, pos, f, g, adj, scatter=True)
+    _bar("antialias d pos", dp, lambda o, x, t: o.antialias_bwd(color, rast, x[0], f, x[1], adj, scatter=True, terms=t)[1], [pos, g], seed)
     assert (dp[pos[..., 3] <= 0] == 0).all()
 
     c1, p1 = _t(dev, color).requires_grad_(True), _t(dev, pos)
@@ -91,7 +91,8 @@ def _check_antialias(dev, f, pos, rast, C, seed, poison=False):
     assert same_bits(c1.grad.cpu().numpy(), dc32)
     c2, p2 = _t(dev, color), _t(dev, pos).requires_grad_(True)
     antialias(c2, rt, p2, ft, topo).backward(gt)                         # d pos alone
-    assert rel_l2(p2.grad.cpu().numpy(), dp) <= 1e-6
+    aa_bwd = lambda o, x, t: o.antialias_bwd(color, rast, x[0], f, x[1], adj, scatter=True, terms=t)[1]
+    _bar("antialias d pos (d pos alone)", p2.grad.cpu().numpy(), aa_bwd, [pos, g], seed)
     if not (rast[..., 3] > 0).any():                                     # an empty image passes through untouched
         assert same_bits(got, color) and same_bits(dc, g) and (dp == 0).all()
     if poison:
@@ -104,9 +105,9 @@ def _check_antialias(dev, f, pos, rast, C, seed, poison=False):
 
 
 def _check_rasterize_bwd(dev, ctx, m, res, k, pos, f, rast, seed):
-    """d pos of layer k from d rast alone, from d rast + d rast_db and from d rast_db alone, at the fp64 bar against raster_bwd and
-    rast_db_bwd; random z/w and id channels in d rast change nothing; an upstream gradient zero on a checkerboard of pixels."""
-    g32, g64 = geometry_oracle(), geometry_oracle(f64=True)
+    """d pos of layer k from d rast alone, from d rast + d rast_db and from d rast_db alone, per element against raster_bwd and
+    rast_db_bwd of the fp64 oracle; random z/w and id channels in d rast change nothing; an upstream gradient zero on a checkerboard of
+    pixels.  With both upstream gradients the statistics of the two scatters add."""
     rng = np.random.default_rng(seed)
     B, H, W = rast.shape[:3]
     g_any = rng.standard_normal((B, H, W, 4)).astype(np.float32)
@@ -129,30 +130,18 @@ def _check_rasterize_bwd(dev, ctx, m, res, k, pos, f, rast, seed):
             torch.autograd.backward(ts, gs)
         return p.grad.cpu().numpy()
 
-    for gg in (g, g_chk):
-        _fp64_bar(run(gg), g32.raster_bwd(pos, f, rast, gg), g64.raster_bwd(pos, f, rast, gg), "rasterize d pos")
-    assert rel_l2(run(g_any), run(g)) <= 1e-6
-    _fp64_bar(run(g, h), g32.raster_bwd(pos, f, rast, g) + g32.rast_db_bwd(pos, f, rast, h),
-              g64.raster_bwd(pos, f, rast, g) + g64.rast_db_bwd(pos, f, rast, h), "rasterize_db d pos")
-    _fp64_bar(run(None, h), g32.rast_db_bwd(pos, f, rast, h), g64.rast_db_bwd(pos, f, rast, h), "rasterize_db d pos (rast_db only)")
-
-
-def _interp_dattr(attr, f, rast, g, dt):
-    """d attr of interpolate, scattered in numpy in `dt`: vertex k of the pixel's triangle gets its barycentric times g"""
-    ids = rast[..., 3].astype(np.int64) - 1
-    m = (ids >= 0) & (ids < f.shape[0])
-    u, v = rast[..., 0][m].astype(dt), rast[..., 1][m].astype(dt)
-    w = np.stack([u, v, (dt(1) - u) - v], -1)
-    gg, tri = g[m].astype(dt), f[ids[m]]
-    d = np.zeros(attr.shape, dt)
-    for k in range(3):
-        np.add.at(d, (np.nonzero(m)[0], tri[:, k]) if attr.ndim == 3 else tri[:, k], w[:, k, None] * gg)
-    return d
+    r_bwd = lambda o, x, t: o.raster_bwd(x[0], f, rast, x[1], terms=t)
+    db_bwd = lambda o, x, t: o.rast_db_bwd(x[0], f, rast, x[1], terms=t)
+    for gg, what in ((g, "rasterize d pos"), (g_chk, "rasterize d pos (checkerboard)")):
+        _bar(what, run(gg), r_bwd, [pos, gg], seed)
+    _bar("rasterize d pos (random z/w, id)", run(g_any), r_bwd, [pos, g], seed)
+    _bar("rasterize_db d pos", run(g, h), lambda o, x, t: r_bwd(o, x[:2], t) + db_bwd(o, [x[0], x[2]], t), [pos, g, h], seed)
+    _bar("rasterize_db d pos (rast_db only)", run(None, h), db_bwd, [pos, h], seed)
 
 
 def _check_interpolate(dev, f, rast, V, seed, chans=(1, 5, 9)):
     """forward and d rast bit for bit against the fp32 oracle for [V,C] and [B,V,C] attributes (d rast the same without attr requiring
-    grad), d attr at the fp64 bar"""
+    grad), d attr per element against the fp64 oracle"""
     from nvdiffrecmc_b200.raster import interpolate
     g32 = geometry_oracle()
     rng = np.random.default_rng(seed)
@@ -171,8 +160,8 @@ def _check_interpolate(dev, f, rast, V, seed, chans=(1, 5, 9)):
             r2 = rt.clone().requires_grad_(True)
             interpolate(_t(dev, attr), r2, ft)[0].backward(_t(dev, g))
             assert same_bits(r2.grad.cpu().numpy(), dr)
-            _fp64_bar(a.grad.cpu().numpy(), _interp_dattr(attr, f, rast, g, np.float32), _interp_dattr(attr, f, rast, g, np.float64),
-                      "interpolate d attr")
+            _bar("interpolate d attr C=%d%s" % (Cn, " [B,V,C]" if batched else ""), a.grad.cpu().numpy(),
+                 lambda o, x, t: o.interpolate_bwd_attr(attr.shape, f, rast, x[0], terms=t), [g], seed)
 
 
 def _run(dev, v, f, mtx, res, layers=(0,), C=4, T=None, pos=None, seed=0, chans=(1, 5, 9), poison=False):

@@ -1,14 +1,14 @@
 """GPU: the fused MLP texture (csrc/mlptexture.cu, nvdiffrecmc_b200.mlptexture.MLPTexture3D) against the fp32 CPU oracle -- output, saved
-encoding, d texc and d W bit for bit, d params to the atomics' summation order -- on edge inputs and at the chunk boundaries of d W; plus
-the drop-in's reproduction of the reference's MLPTexture3D, its initialisation, needs_input_grad, no_grad, CUDA-graph replay and a small
-training run."""
+encoding, d texc and d W bit for bit, d params per element within the bound of two summation orders of the same fp32 terms -- on edge
+inputs and at the chunk boundaries of d W; plus the drop-in's reproduction of the reference's MLPTexture3D, its initialisation,
+needs_input_grad, no_grad, CUDA-graph replay and a small training run."""
 import os
 
 import numpy as np
 import pytest
 import torch
 
-from common import rel_l2
+from common import check_scatter_fp32, rel_l2
 from oracle.hashgrid import REF_CONFIG
 from oracle.mlptexture import MLPTEX_CHUNK, mlptexture_oracle
 from nvdiffrecmc_b200 import _lib as L
@@ -76,12 +76,20 @@ def _oracle(tex, t, g):
     return out, enc, dt, dp * 128, dw, lv
 
 
-def _check_dparams(dp, ref, lv):
-    assert np.array_equal(dp == 0, ref == 0)
-    for l in range(lv["n_levels"]):
-        a, b = 2 * int(lv["offset"][l]), 2 * int(lv["offset"][l + 1])
-        if np.any(ref[a:b]):
-            assert rel_l2(dp[a:b], ref[a:b]) <= 1e-5, l
+def _dp_stats(tex, t, g):
+    """(abs sum x 128, count) of the fp32 oracle's d params terms, in the units of the kernel's gradient (the reference's x128)"""
+    o = mlptexture_oracle()
+    lv = o.levels(REF_CONFIG)
+    ws = [_np(w) for w in tex.net.weights()]
+    p = _np(tex.encoder.params)
+    a = o.mlptex_backward(t, AABB, _mm(tex), p, lv, ws, g, want_t=False, want_w=False, terms="abs")[0]
+    n = o.mlptex_backward(t, AABB, _mm(tex), p, lv, ws, g, want_t=False, want_w=False, terms="count")[0]
+    return a * 128, n
+
+
+def _check_dparams(dp, ref, stats, what="d params"):
+    """d params per element: the kernel adds the fp32 oracle's terms w_c d e (x128) in another order"""
+    check_scatter_fp32(what, dp, ref, stats[0], stats[1], tag="mlptexture")
 
 
 def _saved_encoding(out):
@@ -105,7 +113,7 @@ def test_bit_identical_to_the_oracle(dev, n, C, hidden):
     assert np.array_equal(_np(dt), r_dt)
     for a, b in zip(dw, r_dw):
         assert np.array_equal(_np(a), b)
-    _check_dparams(_np(dp), r_dp, lv)
+    _check_dparams(_np(dp), r_dp, _dp_stats(tex, t, g), "d params n=%d C=%d hidden=%d" % (n, C, hidden))
 
 
 def test_nonfinite_points_match_the_oracle_where_finite(dev):
@@ -124,7 +132,9 @@ def test_nonfinite_points_match_the_oracle_where_finite(dev):
         assert np.array_equal(_np(a), b, equal_nan=True)
     fin = np.isfinite(r_dp)
     assert np.array_equal(np.isfinite(_np(dp)), fin)
-    _check_dparams(np.where(fin, _np(dp), 0), np.where(fin, r_dp, 0), lv)
+    a, cnt = _dp_stats(tex, t, g)
+    _check_dparams(np.where(fin, _np(dp), 0), np.where(fin, r_dp, 0), (np.where(fin, a, 0), np.where(fin, cnt, 0)),
+                   "d params, non-finite points")
 
 
 def test_dead_relus_give_exactly_zero_gradients(dev):
@@ -147,7 +157,7 @@ def test_zero_upstream_gradient_points_add_nothing(dev):
     out, dt, dp, dw = _run(tex, t, g, dev)
     r_out, r_enc, r_dt, r_dp, r_dw, lv = _oracle(tex, t, g)
     assert not dt[::2].any()
-    _check_dparams(_np(dp), r_dp, lv)
+    _check_dparams(_np(dp), r_dp, _dp_stats(tex, t, g), "d params, zero-gradient spot")
     only_spot = (_oracle(tex, t[:1], np.ones((1, 6), np.float32))[3] != 0) & (_oracle(tex, t[1::2], g[1::2])[3] == 0)
     assert only_spot.any() and not _np(dp)[only_spot].any()
 

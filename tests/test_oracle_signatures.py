@@ -14,7 +14,7 @@ from oracle.mlptexture import MlpTextureOracle
 from oracle.texture import TextureOracle
 
 ORACLE_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
-WRAPPERS = [(Oracle, 48), (GeometryOracle, 14), (HashGridOracle, 4), (TextureOracle, 4), (MlpTextureOracle, 7),
+WRAPPERS = [(Oracle, 48), (GeometryOracle, 15), (HashGridOracle, 4), (TextureOracle, 4), (MlpTextureOracle, 7),
             (DmtetOracle, 9)]     # exports of each library at the time of writing
 
 

@@ -420,6 +420,22 @@ int32_t mcs_chroma_loss_num_partials(int32_t B, int32_t H, int32_t W);
 int mcs_chroma_loss_fwd(const mcs_tensor *kd, const mcs_tensor *color_ref, float lambda_chroma, double *partials, float *loss, mcs_stream stream);
 int mcs_chroma_loss_bwd(const mcs_tensor *kd, const mcs_tensor *color_ref, float lambda_chroma, const float *d_loss, float *d_kd, mcs_stream stream);
 
+/* ---- the jittered regulariser taps of shade() (render/render.py:50-97): kd_grad, ks_grad, normal_grad and perturbed_nrm_grad with alpha
+ *      appended; semantics in csrc/taps.cu.  Operands are fp32 views of rast's B, H, W with any non-negative element strides: rast [..,4],
+ *      jitter [..,2], kd [..,3|4], ks / gb_normal [..,3], perturbed_nrm [..,3] or NULL, kd_jitter [..,kd's C] and ks_jitter [..,3] both
+ *      or both NULL (given: the MLP path, render.py:63-68; else the texture path).  B*H*W < 2^31.
+ *      _fwd overwrites kd_grad [B,H,W,C+1] and ks_grad / normal_grad / perturbed_nrm_grad (when perturbed_nrm is given) [B,H,W,4], dense.
+ *      _bwd reads their dense upstream gradients and adds into d_kd, d_ks, d_gb_normal, d_perturbed_nrm: dense [B,H,W,4] (channel 3 of a
+ *      3-channel operand receives nothing), caller-zeroed, float atomics; it overwrites d_kd_jitter [B,H,W,C] and d_ks_jitter [B,H,W,3]
+ *      (MLP path only).  The [..,4] buffers are 16-byte aligned.  One launch each, no host sync, no allocation. */
+int mcs_jitter_taps_fwd(const mcs_tensor *rast, const mcs_tensor *jitter, const mcs_tensor *kd, const mcs_tensor *ks, const mcs_tensor *gb_normal,
+                        const mcs_tensor *perturbed_nrm, const mcs_tensor *kd_jitter, const mcs_tensor *ks_jitter, float *kd_grad, float *ks_grad,
+                        float *normal_grad, float *perturbed_nrm_grad, mcs_stream stream);
+int mcs_jitter_taps_bwd(const mcs_tensor *rast, const mcs_tensor *jitter, const mcs_tensor *kd, const mcs_tensor *ks, const mcs_tensor *gb_normal,
+                        const mcs_tensor *perturbed_nrm, const mcs_tensor *kd_jitter, const mcs_tensor *ks_jitter, const float *d_kd_grad,
+                        const float *d_ks_grad, const float *d_normal_grad, const float *d_perturbed_nrm_grad, float *d_kd, float *d_ks,
+                        float *d_gb_normal, float *d_perturbed_nrm, float *d_kd_jitter, float *d_ks_jitter, mcs_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

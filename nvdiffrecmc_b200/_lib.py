@@ -17,7 +17,7 @@ _LIBDIR = os.path.join(_PKG, "lib")
 HEADER = os.path.join(os.path.dirname(_PKG), "include", "mcshade.h")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
 SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu",
-           "mlptexture.cu", "dmtet.cu", "regularizer.cu"]
+           "mlptexture.cu", "dmtet.cu", "regularizer.cu", "taps.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 

@@ -56,7 +56,7 @@
 //     NaN bound is returned; lo / hi are read on the device.  One launch.
 //   Normalize (C = 3): x / sqrt(max(dot(x, x), 1e-20)) per texel over every level (util.safe_normalize); dot left to right, NaN kept
 //     through the max.  One launch.
-#include "common.cuh"
+#include "texture.cuh"
 
 // Layout choices, measured with tools/texbench.py on bench.py's shape (8 x 512^2, Texture2D.sample x 3 on 1024^2 chains and the five
 // regulariser taps; one H100 80GB HBM3 at a 400 W power limit, DESIGN.md section 4): a warp covers an 8 x 4 pixel tile (backward of the
@@ -130,26 +130,6 @@ __device__ __forceinline__ Lod tex_lod(const float4 da, float W0, float H0, int 
 // the four taps of one level: element offsets of t00, t10, t01, t11 (texel * C + minibatch offset) and the bilinear fractions
 struct Taps { int64_t o00, o10, o01, o11; float fx, fy; };
 
-// one axis of the taps at texel-space coordinate x (texel centres at integer + 0.5 - 0.5 = integers)
-__device__ __forceinline__ void tex_axis_at(float x, int n, bool clamp, int &i0, int &i1, float &fr)
-{
-    fr = __fsub_rn(x, floorf(x));
-    const int x0 = __float2int_rd(x);                  // cvt.rmi.s32.f32: saturating, NaN -> 0
-    if (clamp) {
-        i0 = min(max(x0, 0), n - 1);
-        i1 = x0 >= n - 1 ? n - 1 : max(x0 + 1, 0);
-    } else {
-        i0 = x0 % n;
-        if (i0 < 0) i0 += n;
-        i1 = i0 + 1 == n ? 0 : i0 + 1;
-    }
-}
-
-__device__ __forceinline__ void tex_axis(float u, int n, bool clamp, int &i0, int &i1, float &fr)
-{
-    tex_axis_at(__fsub_rn(__fmul_rn(u, (float)n), 0.5f), n, clamp, i0, i1, fr);
-}
-
 __device__ __forceinline__ Taps tex_taps(const mcs_texture_levels &lv, int k, int b, float u, float v, bool clamp)
 {
     const int W = lv.w[k], H = lv.h[k], C = lv.C;
@@ -162,8 +142,6 @@ __device__ __forceinline__ Taps tex_taps(const mcs_texture_levels &lv, int k, in
     t.o00 = base + (r0 + x0) * C; t.o10 = base + (r0 + x1) * C; t.o01 = base + (r1 + x0) * C; t.o11 = base + (r1 + x1) * C;
     return t;
 }
-
-template <int VEC> struct Vec { float v[VEC]; };
 
 template <int VEC>
 __device__ __forceinline__ Vec<VEC> ld(const float *p)
@@ -194,25 +172,6 @@ __device__ __forceinline__ Quad<VEC> ld_quad(const float *p, const Taps &t, int 
     return q;
 }
 
-__device__ __forceinline__ float bilerp(float t00, float t10, float t01, float t11, float fx, float fy)
-{
-    const float ox = __fsub_rn(1.0f, fx), oy = __fsub_rn(1.0f, fy);
-    const float top = __fadd_rn(__fmul_rn(ox, t00), __fmul_rn(fx, t10));
-    const float bot = __fadd_rn(__fmul_rn(ox, t01), __fmul_rn(fx, t11));
-    return __fadd_rn(__fmul_rn(oy, top), __fmul_rn(fy, bot));
-}
-
-// d tex of one tap and channel group: one vector reduction (red.global.add.v4/.v2.f32)
-template <int VEC>
-__device__ __forceinline__ void scatter(float *base, int64_t off, Vec<VEC> g, bool live)
-{
-    if (!live) return;
-    float *p = base + off;
-    if (VEC == 4) atomicAdd((float4 *)p, make_float4(g.v[0], g.v[1], g.v[2], g.v[3]));
-    else if (VEC == 2) atomicAdd((float2 *)p, make_float2(g.v[0], g.v[1]));
-    else atomicAdd(p, g.v[0]);
-}
-
 template <int VEC>
 __device__ __forceinline__ void scatter_level(float *grad, const Taps &t, int cg, float wl, const Vec<VEC> &g, bool live)
 {
@@ -229,27 +188,12 @@ __device__ __forceinline__ void scatter_level(float *grad, const Taps &t, int cg
     }
 }
 
-// pixel of this thread: an 8 x 4 tile per warp
-__device__ __forceinline__ bool tex_pixel(const TexArgs &a, int &b, int &y, int &x, int64_t &pix)
-{
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t tx = (a.W + 7) / 8, ty = (a.H + 3) / 4, per = tx * ty;
-    const int64_t w = i >> 5, lane = i & 31;
-    b = (int)(w / per);
-    const int64_t t = w - (int64_t)b * per;
-    y = (int)(t / tx) * 4 + (int)(lane >> 3);
-    x = (int)(t % tx) * 8 + (int)(lane & 7);
-    const bool in = b < a.B && y < a.H && x < a.W;
-    pix = ((int64_t)b * a.H + y) * a.W + x;
-    return in;
-}
-
 template <int VEC>
 __global__ void __launch_bounds__(256) k_texture_fwd(const TexArgs a)
 {
     int b, y, x;
     int64_t pix;
-    if (!tex_pixel(a, b, y, x, pix)) return;
+    if (!tex_pixel(a.B, a.H, a.W, b, y, x, pix)) return;
     const mcs_texture_levels &lv = a.lv;
     const float2 uv = __ldg((const float2 *)a.uv + pix);
     int l0 = 0, l1 = 0;
@@ -298,7 +242,7 @@ __global__ void __launch_bounds__(256) k_texture_bwd(const TexArgs a)
 {
     int b, y, x;
     int64_t pix;
-    const bool in = tex_pixel(a, b, y, x, pix);
+    const bool in = tex_pixel(a.B, a.H, a.W, b, y, x, pix);
     const int64_t p = in ? pix : 0;
     const mcs_texture_levels &lv = a.lv;
     const int tb = in ? b : 0;
@@ -419,7 +363,7 @@ bool aligned_all(const TexArgs &a, int n_levels, uintptr_t mask)
 int tex_launch(const TexArgs &a, cudaStream_t s, bool bwd)
 {
     const int C = a.lv.C;
-    const int64_t n_threads = (int64_t)a.B * ((a.W + 7) / 8) * ((a.H + 3) / 4) * 32;
+    const int64_t n_threads = tex_pixel_threads(a.B, a.H, a.W);
     const unsigned blocks = (unsigned)((n_threads + 255) / 256);
     const int n = a.lv.n_levels;
     if (C % 4 == 0 && aligned_all(a, n, 15)) { if (bwd) k_texture_bwd<4><<<blocks, 256, 0, s>>>(a); else k_texture_fwd<4><<<blocks, 256, 0, s>>>(a); }

@@ -1,6 +1,7 @@
 """The image-space regularisers of both geometry passes on the GPU: drop-ins for the reference's `shading_loss`,
 `material_smoothness_grad` and `chroma_loss` (render/regularizer.py:15-49), run by the kernels of csrc/regularizer.cu (contract stated
-there: torch's conventions for ties of max, clamp boundaries, abs at 0, the sRGB branch and the means' denominators).
+there: torch's conventions for ties of max, clamp boundaries, abs at 0, the sRGB branch and the means' denominators), and
+`jitter_taps`, the producer of their inputs in shade() (render/render.py:50-97), run by the kernels of csrc/taps.cu.
 
 Each function returns a 0-dim fp32 device tensor, as `torch.mean(...) * lambda` does.  Forward and backward are one streaming launch
 each (plus a one-CTA finish in the forward), make no host synchronisation and can be captured in a CUDA graph; the backward reads its
@@ -14,7 +15,7 @@ import torch
 
 from . import _lib as L
 
-__all__ = ["shading_loss", "material_smoothness_grad", "chroma_loss"]
+__all__ = ["shading_loss", "material_smoothness_grad", "chroma_loss", "jitter_taps"]
 
 
 def _check(fn, named, lambdas):
@@ -162,3 +163,105 @@ def chroma_loss(kd, color_ref, lambda_chroma):
     if torch.is_grad_enabled() and kd.requires_grad:
         return _ChromaLoss.apply(kd, color_ref, lambda_chroma)
     return _chroma_fwd(kd.detach(), color_ref, lambda_chroma)
+
+
+# ---- jitter_taps ----
+_TAP_OPERANDS = ("rast", "jitter", "kd", "ks", "gb_normal", "perturbed_nrm", "kd_jitter", "ks_jitter")
+
+
+def _check_taps(named):
+    """ValueError naming the argument unless every given operand is an fp32 CUDA [B,H,W,C] tensor of rast's B, H, W and device with its
+    channel count, kd_jitter / ks_jitter come together and jitter does not require grad.  rast may require grad (rasterize's output is
+    differentiable in the vertices); only its coverage test is read, which has no gradient, as in the reference."""
+    fn = "jitter_taps"
+    rast = named["rast"]
+    if (named["kd_jitter"] is None) != (named["ks_jitter"] is None):
+        raise ValueError("%s: kd_jitter and ks_jitter go together (the MLP path), got only %s" % (
+            fn, "kd_jitter" if named["ks_jitter"] is None else "ks_jitter"))
+    chans = {"rast": (4,), "jitter": (2,), "kd": (3, 4), "ks": (3,), "gb_normal": (3,), "perturbed_nrm": (3,), "ks_jitter": (3,)}
+    given = [(name, named[name]) for name in _TAP_OPERANDS if named[name] is not None or name in ("rast", "jitter", "kd", "ks", "gb_normal")]
+    for name, t in given:
+        if not isinstance(t, torch.Tensor):
+            raise ValueError("%s: %s must be a torch.Tensor, got %s" % (fn, name, type(t).__name__))
+        if t.dtype != torch.float32:
+            raise ValueError("%s: %s must be float32, got %s" % (fn, name, t.dtype))
+        want = chans[name] if name in chans else (named["kd"].shape[3],)      # kd_jitter: kd's channels (kd is checked before it)
+        if t.dim() != 4 or t.shape[3] not in want:
+            raise ValueError("%s: %s must be [B,H,W,%s], got %s" % (fn, name, "|".join(map(str, want)), tuple(t.shape)))
+    for name, t in given:
+        if not t.is_cuda:
+            raise ValueError("%s: %s must be a CUDA tensor, got %s" % (fn, name, t.device))
+        if t.shape[:3] != rast.shape[:3]:
+            raise ValueError("%s: %s has B,H,W %s, rast has %s" % (fn, name, tuple(t.shape[:3]), tuple(rast.shape[:3])))
+        if t.device != rast.device:
+            raise ValueError("%s: %s is on %s, rast on %s" % (fn, name, t.device, rast.device))
+        if any(s >= 2 ** 31 or s < 0 for s in t.stride()):
+            raise ValueError("%s: %s has a stride outside int32" % (fn, name))
+    if named["jitter"].requires_grad:
+        raise ValueError("%s: jitter is a constant and must not require grad (its gradient would be dropped)" % fn)
+    if rast.shape[0] * rast.shape[1] * rast.shape[2] >= 2 ** 31:
+        raise ValueError("%s: at most 2^31 - 1 pixels" % fn)
+
+
+def _desc(t):
+    return None if t is None else L.nhwc(t)
+
+
+def _taps_fwd(ops):
+    rast, kd, pn = ops[0], ops[2], ops[5]
+    B, H, W = rast.shape[:3]
+    dev = rast.device
+    outs = [torch.empty(B, H, W, kd.shape[3] + 1, dtype=torch.float32, device=dev)]
+    outs += [torch.empty(B, H, W, 4, dtype=torch.float32, device=dev) for _ in range(2 if pn is None else 3)]
+    if B * H * W:
+        descs = [_desc(t) for t in ops]
+        L.check(L.lib().mcs_jitter_taps_fwd(*descs, *[o.data_ptr() for o in outs], *([None] if pn is None else []), L.stream_ptr()),
+                "jitter_taps_fwd")
+    return outs
+
+
+class _JitterTaps(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, *ops):
+        ctx.has_pn, ctx.mlp = ops[5] is not None, ops[6] is not None
+        ctx.save_for_backward(*ops)
+        return tuple(_taps_fwd(ops))
+
+    @staticmethod
+    def backward(ctx, *d_outs):
+        ops = ctx.saved_tensors
+        rast, kd = ops[0], ops[2]
+        B, H, W = rast.shape[:3]
+        dev = rast.device
+        ckd = kd.shape[3]
+        grads4 = [torch.zeros(B, H, W, 4, dtype=torch.float32, device=dev) for _ in range(4 if ctx.has_pn else 3)]
+        gj = [torch.empty(B, H, W, ckd, dtype=torch.float32, device=dev), torch.empty(B, H, W, 3, dtype=torch.float32, device=dev)] \
+            if ctx.mlp else [None, None]
+        ups = [g.to(torch.float32).contiguous() for g in d_outs]
+        if B * H * W:
+            ptr = lambda t: None if t is None else t.data_ptr()
+            L.check(L.lib().mcs_jitter_taps_bwd(*[_desc(t) for t in ops], *[u.data_ptr() for u in ups], *([None] if not ctx.has_pn else []),
+                                                *[g.data_ptr() for g in grads4], *([None] if not ctx.has_pn else []), ptr(gj[0]), ptr(gj[1]),
+                                                L.stream_ptr()), "jitter_taps_bwd")
+        d_kd = grads4[0] if ckd == 4 else grads4[0][..., :3]
+        d = [None, None, d_kd, grads4[1][..., :3], grads4[2][..., :3], grads4[3][..., :3] if ctx.has_pn else None, gj[0], gj[1]]
+        return tuple(g if need else None for g, need in zip(d, ctx.needs_input_grad))
+
+
+def jitter_taps(rast, jitter, kd, ks, gb_normal, perturbed_nrm=None, kd_jitter=None, ks_jitter=None):
+    """The jittered regulariser differences of the reference's shade() (render/render.py:50-97), one launch each way: -> {"kd_grad":
+    [B,H,W,Ckd+1], "ks_grad", "normal_grad" and, when perturbed_nrm is given, "perturbed_nrm_grad": [B,H,W,4]}, each with shade()'s
+    alpha appended, ready for its `buffers` dict.
+
+    rast [B,H,W,4] and jitter [B,H,W,2] (pixel_grid + the caller's offset draw) are constants; kd [B,H,W,3|4], ks, gb_normal and
+    perturbed_nrm [B,H,W,3], any strides.  With kd_jitter and ks_jitter (the MLP texture's jittered sample, all_tex_jitter[...,0:3] /
+    [...,3:6]) the differences are the MLP path's (no tap, no grad weight); else kd and ks are tapped at jitter.  Differentiable in kd,
+    ks, gb_normal, perturbed_nrm, kd_jitter and ks_jitter."""
+    ops = (rast, jitter, kd, ks, gb_normal, perturbed_nrm, kd_jitter, ks_jitter)
+    _check_taps(dict(zip(_TAP_OPERANDS, ops)))
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in ops):
+        outs = _JitterTaps.apply(*ops)
+    else:
+        outs = _taps_fwd(tuple(None if t is None else t.detach() for t in ops))
+    names = ["kd_grad", "ks_grad", "normal_grad", "perturbed_nrm_grad"]
+    return dict(zip(names, outs))

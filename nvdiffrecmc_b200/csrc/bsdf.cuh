@@ -159,11 +159,13 @@ __device__ __forceinline__ f3 fwd_pbr_specular(f3 col, f3 nrm, f3 wo, f3 wi, flo
     f3 F = fwd_fresnel3(col, F3(1.0f), woDotH);
     return F * (D * G * 0.25f / woDotN);
 }
-__device__ __forceinline__ void bwd_pbr_specular(f3 col, f3 nrm, f3 wo, f3 wi, float alpha, float min_roughness,
-                                                 f3 &d_col, f3 &d_nrm, f3 &d_wo, f3 &d_wi, float &d_alpha, f3 d_out)
+// Accumulates the adjoint of d_out and returns the lobe's value, fwd_pbr_specular's operations on the same intermediates (half vector,
+// cosines, D, G, F and the lambda terms are evaluated once for both); callers that need only the adjoint ignore the value.
+__device__ __forceinline__ f3 bwd_pbr_specular(f3 col, f3 nrm, f3 wo, f3 wi, float alpha, float min_roughness,
+                                               f3 &d_col, f3 &d_nrm, f3 &d_wo, f3 &d_wi, float &d_alpha, f3 d_out)
 {
     float woDotN = dot_exact(wo, nrm), wiDotN = dot_exact(wi, nrm);
-    if (!((woDotN > MCS_SPEC_EPS) & (wiDotN > MCS_SPEC_EPS))) return;
+    if (!((woDotN > MCS_SPEC_EPS) & (wiDotN > MCS_SPEC_EPS))) return F3(0.0f);
     float a = clampf(alpha, __fmul_rn(min_roughness, min_roughness), 1.0f);
     float alphaSqr = __fmul_rn(a, a);
     f3 hsum = F3(__fadd_rn(wo.x, wi.x), __fadd_rn(wo.y, wi.y), __fadd_rn(wo.z, wi.z));
@@ -193,6 +195,7 @@ __device__ __forceinline__ void bwd_pbr_specular(f3 col, f3 nrm, f3 wo, f3 wi, f
     d_wo += d_hsum;
     d_wi += d_hsum;
     if (alpha > min_roughness * min_roughness) d_alpha += d_alphaSqr * 2.0f * alpha;
+    return F * (D * G * 0.25f / woDotN);
 }
 
 // ---- in-kernel flavour (optixutils/c_src/bsdf.h:222-275): diffuse is a demodulated scalar ----
@@ -203,16 +206,25 @@ __device__ __forceinline__ void ox_fwd_pbr_bsdf(f3 kd, f3 arm, f3 wo, f3 nrm, f3
     diffuse = fwd_lambert(nrm, wi);
     specular = fwd_pbr_specular(spec_color(kd, arm), nrm, wo, wi, __fmul_rn(arm.y, arm.y), min_roughness);
 }
+// Value and adjoint in one pass, for the backward passes, which need both (the value weights the light gradient): diffuse / specular
+// are ox_fwd_pbr_bsdf's value, with the FMAs of the Lambert dot product spelled out so that it rounds the same wherever the body is
+// inlined (the lobe's one FMA, in Fresnel, has no other way to contract), and the adjoints of d_diffuse / d_specular are accumulated
+// into d_kd, d_arm, d_wo, d_nrm.
+// diffuse_only: Lambert alone (BSDF 'diffuse' and 'white'), which has no kd, arm or wo adjoint.
 // d_wo is returned so the caller can push it through wo = normalize(view_pos - pos) once per pixel
 // (the map is linear in d_wo, so summing d_wo over samples first is exact up to rounding).
-__device__ __forceinline__ void ox_bwd_pbr_bsdf(f3 kd, f3 arm, f3 wo, f3 nrm, f3 wi, float min_roughness,
-                                                f3 &d_kd, f3 &d_arm, f3 &d_wo, f3 &d_nrm, float d_diffuse, f3 d_specular)
+__device__ __forceinline__ void ox_fwdbwd_pbr_bsdf(bool diffuse_only, f3 kd, f3 arm, f3 wo, f3 nrm, f3 wi, float min_roughness, float d_diffuse,
+                                                   f3 d_specular, float &diffuse, f3 &specular, f3 &d_kd, f3 &d_arm, f3 &d_wo, f3 &d_nrm)
 {
-    f3 sc = spec_color(kd, arm);
+    const float nDotWi = __fmaf_rn(nrm.z, wi.z, __fmaf_rn(nrm.x, wi.x, __fmul_rn(nrm.y, wi.y)));     // dot(nrm, wi) as fwd_lambert contracts it
+    diffuse = fmaxf(nDotWi * MCS_INV_PI, 0.0f);
+    specular = F3(0.0f);
     float d_alpha = 0.0f;
     f3 d_sc = F3(0.0f), d_wi = F3(0.0f);
-    bwd_pbr_specular(sc, nrm, wo, wi, __fmul_rn(arm.y, arm.y), min_roughness, d_sc, d_nrm, d_wo, d_wi, d_alpha, d_specular);
-    bwd_lambert(nrm, wi, d_nrm, d_wi, d_diffuse);
+    if (!diffuse_only)
+        specular = bwd_pbr_specular(spec_color(kd, arm), nrm, wo, wi, __fmul_rn(arm.y, arm.y), min_roughness, d_sc, d_nrm, d_wo, d_wi, d_alpha, d_specular);
+    if (nDotWi > 0.0f) bwd_dot(nrm, wi, d_nrm, d_wi, d_diffuse * MCS_INV_PI);                        // bwd_lambert
+    if (diffuse_only) return;
     d_kd -= d_sc * ((arm.x - 1.0f) * arm.z);
     d_arm.x += sum(d_sc * ((F3(0.04f) - kd) * arm.z - F3(0.04f)));
     d_arm.z -= sum(d_sc * (kd - F3(0.04f))) * (arm.x - 1.0f);

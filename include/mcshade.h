@@ -277,6 +277,23 @@ int mcs_antialias_bwd(const float *color, int32_t C, const float *rast, int32_t 
 
 /* Nearest-texel fetch out[i,:] = tex[idx[i],:] (tex [T,C] contiguous, idx int64 [n]; out-of-range indices give zeros) and its scatter-add
  * backward into a caller-zeroed d_tex [T,C] (float atomics) -- the material look-up of the synthetic G-buffer producer. */
+/* ---- layer compositing: render_mesh's composite_buffer (render/render.py:284-291), run for every buffer key at :321-330, for all n_buffers
+ *      buffers of one depth-peel layer in one launch; semantics in csrc/composite.cu.  Every table holds n_buffers (1..16) mcs_tensor
+ *      views of [B,H,W,C_k] fp32 device memory with any non-negative element strides, B, H, W those of buffers[0] and C_k >= 1 that of
+ *      buffers[k].  rast [B,H,W,4] contiguous; pos / tris / adj as mcs_antialias_fwd.
+ *      _fwd: accum_out[k] = antialias(lerp(accum_in[k], (buffers[k][..C_k-2], 1), mask * buffers[k][C_k-1])), written through the views'
+ *      pointers (every entry given); an accum_in entry with a null pointer reads as zeros.  Layers go back to front, each layer's
+ *      accum_in the previous layer's accum_out (the backgrounds for the deepest).
+ *      _bwd: reads d_accum_out (every entry given) and overwrites d_accum_in and d_buffers (entries with a null pointer are not written);
+ *      adds into d_pos (same layout as pos, caller-zeroed, float atomics; may be null).  Layers go front to back.
+ *      One launch each, no host sync, no allocation. */
+#define MCS_COMPOSITE_MAX_BUFFERS 16
+int mcs_composite_fwd(int32_t n_buffers, const mcs_tensor *buffers, const mcs_tensor *accum_in, const mcs_tensor *accum_out, const float *rast,
+                      const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const int32_t *adj, mcs_stream stream);
+int mcs_composite_bwd(int32_t n_buffers, const mcs_tensor *buffers, const mcs_tensor *accum_in, const mcs_tensor *d_accum_out,
+                      const mcs_tensor *d_accum_in, const mcs_tensor *d_buffers, const float *rast, const float *pos, int64_t pos_batch_stride,
+                      int32_t V, const int32_t *tris, int32_t T, const int32_t *adj, float *d_pos, mcs_stream stream);
+
 int mcs_texel_fetch_fwd(const float *tex, int64_t T, int32_t C, const int64_t *idx, int64_t n, float *out, mcs_stream stream);
 int mcs_texel_fetch_bwd(int64_t T, int32_t C, const int64_t *idx, int64_t n, const float *d_out, float *d_tex, mcs_stream stream);
 
@@ -396,8 +413,9 @@ int mcs_sdf_reg_bwd(const float *sdf, int64_t sdf_stride, int32_t V, const int32
 
 /* ---- image-space regularisers: shading_loss, material_smoothness_grad and chroma_loss (render/regularizer.py:15-49); semantics, and the
  *      torch conventions they keep (ties of max, clamp boundaries, abs at 0, the sRGB branch, the means' denominators), in
- *      csrc/regularizer.cu.  Every operand is an fp32 [B,H,W,4] view with any non-negative element strides; all operands of one call have
- *      the same B, H and W, and B*H*W < 2^31.  lambda_* by value (the fp32 rounding of the reference's Python float).
+ *      csrc/regularizer.cu.  Every operand is an fp32 [B,H,W,4] view with any non-negative element strides, except material_smoothness_grad's
+ *      kd_grad, which may be [B,H,W,5] (luma from channels 0..2, alpha from channel 4; d_kd_grad is then dense [B,H,W,5] with channel 3 = 0
+ *      and needs no alignment); all operands of one call have the same B, H and W, and B*H*W < 2^31.  lambda_* by value (the fp32 rounding of the reference's Python float).
  *      _fwd writes the loss (one float on the device) through `partials`: mcs_<name>_num_partials(B,H,W) x K doubles of device scratch,
  *      K = 3 for shading_loss and material_smoothness_grad, 1 for chroma_loss; the sums are fixed-order, so two runs give the same bits.
  *      shading_loss_fwd also writes means (two floats on the device) = (mean of diffuse luma, mean of specular luma), which its backward

@@ -17,7 +17,7 @@ _LIBDIR = os.path.join(_PKG, "lib")
 HEADER = os.path.join(os.path.dirname(_PKG), "include", "mcshade.h")
 LIB_PATH = os.environ.get("MCS_LIB", os.path.join(_LIBDIR, "libmcshade.so"))     # MCS_LIB: developer override (kernel variants)
 SOURCES = ["core.cu", "elementwise.cu", "denoise.cu", "bvh.cu", "envshade.cu", "lossmesh.cu", "light.cu", "raster.cu", "hashgrid.cu", "texture.cu",
-           "mlptexture.cu", "dmtet.cu", "regularizer.cu", "taps.cu"]
+           "mlptexture.cu", "dmtet.cu", "regularizer.cu", "taps.cu", "composite.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-Xcompiler", "-fPIC"]
 
 
@@ -140,7 +140,7 @@ _KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow"
                      "antialias_topology": 2, "hashgrid_bwd_both": 2, "mlptex_bwd_dw": 2,
                      "texture_fwd": 1, "texture_bwd": 1, "dmtet_count": 1, "dmtet_emit": 1, "dmtet_bwd": 1, "sdf_reg_fwd": 2, "sdf_reg_bwd": 1,
                      "shading_loss_fwd": 2, "material_smoothness_grad_fwd": 2, "chroma_loss_fwd": 2,
-                     "mip_chain_bwd": 1, "mip_clamp": 1, "mip_normalize": 1}     # mip_chain_fwd: mcs_mip_chain_fwd_launches(n_levels)
+                     "mip_chain_bwd": 1, "mip_clamp": 1, "mip_normalize": 1, "composite_fwd": 1, "composite_bwd": 1}     # mip_chain_fwd: mcs_mip_chain_fwd_launches(n_levels)
 
 
 def check(status, what, launches=None):

@@ -82,6 +82,7 @@
 //                          e_f and e_o have strictly opposite signs; the smallest t of the candidate edges wins;
 //                       6. blend: o gains max(0, t - 1/2) (c_f - c_o), f gains max(0, 1/2 - t) (c_o - c_f); a pixel's <= 4 pairs add
 //                          in the fixed order left, right, up, down.
+//                     The pair logic (rules 1-5 and the d pos scatter) is csrc/antialias.cuh, shared with csrc/composite.cu.
 //                     The forward is a per-pixel gather (each thread evaluates its own <= 4 pairs), so it is bit-deterministic without
 //                     colour atomics.  The backward gathers d color the same way; d pos (dt/d(x, y, w) of the crossing edge's endpoints,
 //                     dt/de_f = -e_o / D^2, dt/de_o = e_f / D^2 with D = e_f - e_o) is scattered with float atomics by the pixel that owns
@@ -96,6 +97,7 @@
 //                     d pos is an order-dependent float-atomic sum, within float rounding of the oracle's scatter.
 #include "ctx.h"
 #include "bvh_traverse.cuh"
+#include "antialias.cuh"
 
 namespace {
 
@@ -111,12 +113,6 @@ __device__ __forceinline__ void mul4(const float *__restrict__ m, float x, float
 {
 #pragma unroll
     for (int r = 0; r < 4; ++r) o[r] = fmaf(__ldg(m + 4 * r), x, fmaf(__ldg(m + 4 * r + 1), y, fmaf(__ldg(m + 4 * r + 2), z, __ldg(m + 4 * r + 3) * w)));
-}
-
-// image b, row iy and column ix of flat pixel index i of a [B,H,W] image
-__device__ __forceinline__ void px_decode(int64_t i, int H, int W, int &b, int &iy, int &ix)
-{
-    ix = (int)(i % W); const int64_t t = i / W; iy = (int)(t % H); b = (int)(t / H);
 }
 
 __global__ void __launch_bounds__(128) k_rasterize(const RasterParams p)
@@ -313,18 +309,6 @@ struct RastBwdParams {
     const float4 *drast_db;      // k_rasterize_bwd<true>: d rast_db (drast may then be null)
     float4 *rast_db;             // k_rast_db: output
 };
-
-// NDC coordinate of pixel centre i of n (image row iy -> NDC y = (iy + 0.5) / H * 2 - 1, as k_rasterize), explicitly rounded
-__device__ __forceinline__ float px_ndc(int i, int n) { return __fsub_rn(__fmul_rn(__fdiv_rn(__fadd_rn((float)i, 0.5f), (float)n), 2.0f), 1.0f); }
-
-// a = (x - px w, y - py w) of clip-space vertex (x, y, w) seen from NDC point (px, py), explicitly rounded
-__device__ __forceinline__ float2 clip_a(float x, float y, float w, float px, float py)
-{
-    return make_float2(__fsub_rn(x, __fmul_rn(px, w)), __fsub_rn(y, __fmul_rn(py, w)));
-}
-
-// edge function a_A x a_B, explicitly rounded
-__device__ __forceinline__ float clip_edge(float2 a, float2 b) { return __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x)); }
 
 // triangle id of the clip-space mesh seen from pixel centre (px, py) (file header): vertex ids, (x, y, w), a_k, s_k = a_{k+1} x a_{k+2}
 // and S = (s0 + s1) + s2
@@ -524,166 +508,38 @@ static uint64_t aa_topo_capacity(int32_t T)
 // antialias
 // ------------------------------------------------------------------------------------------------------------------------------------
 struct AAParams {
+    AAGeom g;
     const float *color; int C;
-    const float4 *rast; int B, H, W;
-    const float *pos; int64_t pos_bs; int V;
-    const int32_t *tris; int T;
-    const int32_t *adj;
     float *out;
     const float *dout; float *dcolor, *dpos;
     int64_t npx;
 };
 
-struct AAEdge {
-    float t, ef, eo;
-    int va, vb;
-    float3 A, B;          // (x, y, w) of the edge's endpoints
-};
-
-__device__ __forceinline__ float3 aa_vert(const float *P, int v)
-{
-    const float *q = P + 4 * (size_t)v;
-    return make_float3(__ldg(q), __ldg(q + 1), __ldg(q + 3));
-}
-
-// homogeneous edge function a_A x a_B at NDC point (px, py)
-__device__ __forceinline__ float aa_edge(float3 A, float3 B, float px, float py)
-{
-    return clip_edge(clip_a(A.x, A.y, A.z, px, py), clip_a(B.x, B.y, B.z, px, py));
-}
-
-// facing: det[[x0,y0,w0],[x1,y1,w1],[x2,y2,w2]] > 0
-__device__ __forceinline__ bool aa_facing(float3 a, float3 b, float3 c)
-{
-    const float m0 = __fsub_rn(__fmul_rn(b.y, c.z), __fmul_rn(b.z, c.y));
-    const float m1 = __fsub_rn(__fmul_rn(b.x, c.z), __fmul_rn(b.z, c.x));
-    const float m2 = __fsub_rn(__fmul_rn(b.x, c.y), __fmul_rn(b.y, c.x));
-    return __fadd_rn(__fsub_rn(__fmul_rn(a.x, m0), __fmul_rn(a.y, m1)), __fmul_rn(a.z, m2)) > 0.0f;
-}
-
-// Closest crossing silhouette edge of front triangle F between pixel centres f and o (rules 3-5 of the file header).
-__device__ bool aa_search(const AAParams &p, const float *P, int F, bool horiz, float fx, float fy, float ox, float oy, AAEdge &e)
-{
-    int vi[3];
-    float3 q[3];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) { vi[k] = __ldg(p.tris + 3 * (size_t)F + k); q[k] = aa_vert(P, vi[k]); }
-    int facing = -1;
-    bool found = false;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const int k1 = k == 2 ? 0 : k + 1;
-        const float3 A = q[k], B = q[k1];
-        if (!(A.z > 0.0f && B.z > 0.0f)) continue;
-        const int nb = __ldg(p.adj + 3 * (size_t)F + k);
-        if (nb >= 0 && nb < p.T) {
-            if (facing < 0) facing = aa_facing(q[0], q[1], q[2]) ? 1 : 0;
-            const int n0 = __ldg(p.tris + 3 * (size_t)nb), n1 = __ldg(p.tris + 3 * (size_t)nb + 1), n2 = __ldg(p.tris + 3 * (size_t)nb + 2);
-            if ((aa_facing(aa_vert(P, n0), aa_vert(P, n1), aa_vert(P, n2)) ? 1 : 0) == facing) continue;
-        }
-        const float dX = __fmul_rn(__fsub_rn(__fdiv_rn(B.x, B.z), __fdiv_rn(A.x, A.z)), (float)p.W);
-        const float dY = __fmul_rn(__fsub_rn(__fdiv_rn(B.y, B.z), __fdiv_rn(A.y, A.z)), (float)p.H);
-        if ((fabsf(dY) >= fabsf(dX)) != horiz) continue;
-        const float ef = aa_edge(A, B, fx, fy), eo = aa_edge(A, B, ox, oy);
-        if (!((ef > 0.0f && eo < 0.0f) || (ef < 0.0f && eo > 0.0f))) continue;
-        const float t = __fdiv_rn(ef, __fsub_rn(ef, eo));
-        if (!found || t < e.t) { found = true; e.t = t; e.ef = ef; e.eo = eo; e.va = vi[k]; e.vb = vi[k1]; e.A = A; e.B = B; }
-    }
-    return found;
-}
-
-__device__ __forceinline__ int aa_tid(float4 r, int T)
-{
-    const int id = (int)r.w - 1;
-    return id < T ? id : -1;
-}
-
-// Pair (this pixel p, neighbour q): true when the pair has a crossing edge with a nonzero blend weight w; gain_self tells whether p
-// (else q) gains w * (c_other - c_self); p_front whether p is the front pixel.
-__device__ __forceinline__ bool aa_pair(const AAParams &p, const float *P, float px, float py, int tp, float zp, float qx, float qy, int tq, float zq,
-                                        bool horiz, float &w, bool &gain_self, bool &p_front, AAEdge &e)
-{
-    if (tp == tq) return false;
-    bool pf;
-    if (tq < 0) pf = true;
-    else if (tp < 0) pf = false;
-    else if (zp < zq) pf = true;
-    else if (zq < zp) pf = false;
-    else pf = tp < tq;
-    const bool found = pf ? aa_search(p, P, tp, horiz, px, py, qx, qy, e) : aa_search(p, P, tq, horiz, qx, qy, px, py, e);
-    if (!found) return false;
-    bool gain_front;
-    if (e.t < 0.5f) { w = __fsub_rn(0.5f, e.t); gain_front = true; }
-    else if (e.t > 0.5f) { w = __fsub_rn(e.t, 0.5f); gain_front = false; }
-    else return false;
-    gain_self = gain_front == pf;
-    p_front = pf;
-    return true;
-}
-
-__device__ __forceinline__ void aa_edge_grad(const AAEdge &e, float px, float py, float s, float (&gA)[3], float (&gB)[3])
-{
-    const float ax = e.A.x - px * e.A.z, ay = e.A.y - py * e.A.z, bx = e.B.x - px * e.B.z, by = e.B.y - py * e.B.z;
-    gA[0] += s * by; gA[1] -= s * bx; gA[2] += s * (py * bx - px * by);
-    gB[0] -= s * ay; gB[1] += s * ax; gB[2] += s * (px * ay - py * ax);
-}
-
+// One thread per pixel: its pairs (antialias.cuh), then the blend of every channel as a per-pixel gather.
 template <bool BWD>
 __global__ void __launch_bounds__(256) k_antialias(const AAParams p)
 {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.npx) return;
     int b, iy, ix;
-    px_decode(i, p.H, p.W, b, iy, ix);
-    const float4 r = __ldg(p.rast + i);
-    const int tp = aa_tid(r, p.T);
+    px_decode(i, p.g.H, p.g.W, b, iy, ix);
+    const float4 r = __ldg(p.g.rast + i);
     const int C = p.C;
-    // neighbours in the fixed order left, right, up, down; the right and down pairs are owned by this pixel (d pos scatter)
-    const int nbx[4] = {ix - 1, ix + 1, ix, ix}, nby[4] = {iy, iy, iy - 1, iy + 1};
-    float wk[4];
-    int64_t jk[4];
-    bool selfk[4];
-    int n = 0;
-    const float px = px_ndc(ix, p.W), py = px_ndc(iy, p.H);
-    const float *P = p.pos + (int64_t)b * p.pos_bs;
-#pragma unroll
-    for (int d = 0; d < 4; ++d) {
-        if (nbx[d] < 0 || nbx[d] >= p.W || nby[d] < 0 || nby[d] >= p.H) continue;
-        const int64_t j = i + (nbx[d] - ix) + (int64_t)(nby[d] - iy) * p.W;
-        const float4 rq = __ldg(p.rast + j);
-        const int tq = aa_tid(rq, p.T);
-        if (tq == tp) continue;
-        const float qx = px_ndc(nbx[d], p.W), qy = px_ndc(nby[d], p.H);
-        float w; bool gain_self, p_front; AAEdge e;
-        if (!aa_pair(p, P, px, py, tp, r.z, qx, qy, tq, rq.z, d < 2, w, gain_self, p_front, e)) continue;
-        wk[n] = w; jk[n] = j; selfk[n] = gain_self; ++n;
-        if (BWD && p.dpos && (d == 1 || d == 3)) {
-            // dL/dt of the gaining pixel: o gains (t - 1/2)(c_f - c_o), f gains (1/2 - t)(c_o - c_f)
-            const int64_t gi = gain_self ? i : j, oi = gain_self ? j : i;
-            float dLdt = 0.0f;
-            for (int c = 0; c < C; ++c) dLdt = fmaf(__ldg(p.dout + gi * C + c), __ldg(p.color + oi * C + c) - __ldg(p.color + gi * C + c), dLdt);
-            const bool gain_front = gain_self == p_front;
-            if (gain_front) dLdt = -dLdt;
-            if (dLdt != 0.0f) {
-                const float D = e.ef - e.eo, iD2 = 1.0f / (D * D);
-                const float sf = dLdt * (-e.eo * iD2), so = dLdt * (e.ef * iD2);
-                float gA[3] = {0.0f, 0.0f, 0.0f}, gB[3] = {0.0f, 0.0f, 0.0f};
-                aa_edge_grad(e, p_front ? px : qx, p_front ? py : qy, sf, gA, gB);
-                aa_edge_grad(e, p_front ? qx : px, p_front ? qy : py, so, gA, gB);
-                float *DA = p.dpos + (int64_t)b * p.pos_bs + 4 * (size_t)e.va, *DB = p.dpos + (int64_t)b * p.pos_bs + 4 * (size_t)e.vb;
-                atomicAdd(DA, gA[0]); atomicAdd(DA + 1, gA[1]); atomicAdd(DA + 3, gA[2]);
-                atomicAdd(DB, gB[0]); atomicAdd(DB + 1, gB[1]); atomicAdd(DB + 3, gB[2]);
-            }
-        }
-    }
+    const AAPairs pr = aa_pixel_pairs<BWD>(p.g, i, b, iy, ix, r, p.dpos, [&](bool gain_self, int, int64_t j) {
+        const int64_t gi = gain_self ? i : j, oi = gain_self ? j : i;
+        float dLdt = 0.0f;
+        for (int c = 0; c < C; ++c) dLdt = fmaf(__ldg(p.dout + gi * C + c), __ldg(p.color + oi * C + c) - __ldg(p.color + gi * C + c), dLdt);
+        return dLdt;
+    });
     if (!BWD) {
         const float *cp = p.color + i * C;
         float *o = p.out + i * C;
         for (int c = 0; c < C; ++c) {
             const float cs = __ldg(cp + c);
             float v = cs;
-            for (int k = 0; k < n; ++k)
-                if (selfk[k]) v = __fadd_rn(v, __fmul_rn(wk[k], __fsub_rn(__ldg(p.color + jk[k] * C + c), cs)));
+#pragma unroll
+            for (int d = 0; d < 4; ++d)
+                if (pr.on[d] && pr.self[d]) v = __fadd_rn(v, __fmul_rn(pr.w[d], __fsub_rn(__ldg(p.color + pr.j[d] * C + c), cs)));
             o[c] = v;
         }
     } else if (p.dcolor) {
@@ -693,7 +549,9 @@ __global__ void __launch_bounds__(256) k_antialias(const AAParams p)
         for (int c = 0; c < C; ++c) {
             const float g = __ldg(gp + c);
             float v = g;
-            for (int k = 0; k < n; ++k) v = selfk[k] ? __fmaf_rn(-wk[k], g, v) : __fmaf_rn(wk[k], __ldg(p.dout + jk[k] * C + c), v);
+#pragma unroll
+            for (int d = 0; d < 4; ++d)
+                if (pr.on[d]) v = pr.self[d] ? __fmaf_rn(-pr.w[d], g, v) : __fmaf_rn(pr.w[d], __ldg(p.dout + pr.j[d] * C + c), v);
             dc[c] = v;
         }
     }
@@ -918,8 +776,8 @@ static int aa_common(AAParams &p, const float *color, int32_t C, const float *ra
 {
     MCS_REQUIRE(color && rast && pos && tris && adj && C > 0 && B > 0 && H > 0 && W > 0 && V > 0 && T > 0 && pos_batch_stride >= 0,
                 "mcs_antialias: bad arguments");
-    p.color = color; p.C = C; p.rast = (const float4 *)rast; p.B = B; p.H = H; p.W = W;
-    p.pos = pos; p.pos_bs = pos_batch_stride; p.V = V; p.tris = tris; p.T = T; p.adj = adj;
+    p.color = color; p.C = C;
+    p.g = AAGeom{(const float4 *)rast, B, H, W, pos, pos_batch_stride, V, tris, T, adj};
     p.npx = (int64_t)B * H * W;
     return 0;
 }

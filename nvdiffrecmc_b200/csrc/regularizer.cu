@@ -29,6 +29,8 @@
 //   (not bit-equal to glibc's); this function's gradients are held to a bound, not to bits.
 // material_smoothness_grad (regularizer.py:44-49):
 //   loss = ((fl32(mean_N(luma(kd) * kd.w)) * lkd + fl32(mean_3N(ks.rgb * ks.w)) * lks) + fl32(mean_3N(nrm.rgb * nrm.w)) * lnrm
+//   kd_grad may also have 5 channels (a 4-channel kd with alpha appended, the transparency configuration): luma reads channels 0..2 and
+//   kd.w is the last channel, as the reference's kd_grad[..., -1]; channel 3 gets a gradient of exactly 0 and d kd_grad is [B,H,W,5].
 // chroma_loss (regularizer.py:20-24):
 //   t_c = (kd_c / clamp(value(kd), eps) - ref_c / clamp(value(ref), eps)) * ref.w,  loss = fl32(mean_3N(|t|)) * lc
 //   d kd.w = 0; color_ref is a constant.
@@ -46,10 +48,11 @@ constexpr float SRGB_T = 0.0031308f;
 constexpr float SRGB_E = (float)(1.0 / 2.4);
 constexpr float SRGB_EM1 = (float)(1.0 / 2.4 - 1.0);
 
-struct Op {                      // one [B,H,W,4] operand
+struct Op {                      // one [B,H,W,4] operand (or a 5-channel kd_grad)
     const float *p;
     int64_t s0, s1, s2, s3;      // element strides
-    int vec;                     // dense and 16-byte aligned: one float4 per pixel
+    int64_t sa;                  // element offset of the alpha (last) channel
+    int vec;                     // 4 channels, dense and 16-byte aligned: one float4 per pixel
 };
 
 struct Grid { int H, W, npx; };
@@ -59,7 +62,7 @@ __device__ __forceinline__ float4 ld4(const Op &o, const Grid &g, int px)
     if (o.vec) return __ldg(reinterpret_cast<const float4 *>(o.p) + px);
     const int w = px % g.W, t = px / g.W, h = t % g.H, n = t / g.H;
     const float *q = o.p + n * o.s0 + h * o.s1 + w * o.s2;
-    return make_float4(__ldg(q), __ldg(q + o.s3), __ldg(q + 2 * o.s3), __ldg(q + 3 * o.s3));
+    return make_float4(__ldg(q), __ldg(q + o.s3), __ldg(q + 2 * o.s3), __ldg(q + o.sa));
 }
 
 __device__ __forceinline__ float comp(float4 x, int i) { return i == 0 ? x.x : (i == 1 ? x.y : x.z); }
@@ -239,7 +242,8 @@ __global__ void __launch_bounds__(RG_THREADS) k_shading_bwd(const Op d, const Op
     st4(d_s, px, gs, gs, gs, 0.0f);
 }
 
-__global__ void __launch_bounds__(RG_THREADS) k_smooth_bwd(const Op kd, const Op ks, const Op nr, const Grid g, Lambdas lam,
+// ckd: kd_grad's channel count (4 or 5; d_kd is then dense [B,H,W,ckd])
+__global__ void __launch_bounds__(RG_THREADS) k_smooth_bwd(const Op kd, const Op ks, const Op nr, const Grid g, Lambdas lam, int ckd,
                                                            const float *__restrict__ d_loss, float *__restrict__ d_kd,
                                                            float *__restrict__ d_ks, float *__restrict__ d_nr)
 {
@@ -249,7 +253,12 @@ __global__ void __launch_bounds__(RG_THREADS) k_smooth_bwd(const Op kd, const Op
     const float g1 = mean_grad(G, lam.l0, n1), g2 = mean_grad(G, lam.l1, n3), g3 = mean_grad(G, lam.l2, n3);
     const float4 K = ld4(kd, g, px), S = ld4(ks, g, px), N = ld4(nr, g, px);
     const float gl = __fdiv_rn(__fmul_rn(g1, K.w), 3.0f);
-    st4(d_kd, px, gl, gl, gl, __fmul_rn(g1, luma(K)));
+    if (ckd == 4) {
+        st4(d_kd, px, gl, gl, gl, __fmul_rn(g1, luma(K)));
+    } else {
+        float *q = d_kd + (int64_t)px * 5;
+        q[0] = gl; q[1] = gl; q[2] = gl; q[3] = 0.0f; q[4] = __fmul_rn(g1, luma(K));
+    }
     st4(d_ks, px, __fmul_rn(g2, S.w), __fmul_rn(g2, S.w), __fmul_rn(g2, S.w),
         __fadd_rn(__fadd_rn(__fmul_rn(g2, S.x), __fmul_rn(g2, S.y)), __fmul_rn(g2, S.z)));
     st4(d_nr, px, __fmul_rn(g3, N.w), __fmul_rn(g3, N.w), __fmul_rn(g3, N.w),
@@ -283,12 +292,16 @@ __global__ void __launch_bounds__(RG_THREADS) k_chroma_bwd(const Op kd, const Op
 // ---- host side ----
 int npartials(int64_t npx) { return (int)((npx + RG_CHUNK - 1) / RG_CHUNK); }
 
-// Checks the operand views of one entry (non-null, [B,H,W,4], one shape, non-negative strides, fewer than 2^31 pixels) and fills ops.
-int views(const char *fn, int n, const mcs_tensor *const *v, const char *const *names, Op *ops, Grid &g)
+// Checks the operand views of one entry (non-null, [B,H,W,4] -- operand 0 may have 5 channels when kd5 -- one B, H, W, non-negative
+// strides, fewer than 2^31 pixels) and fills ops.
+int views(const char *fn, int n, const mcs_tensor *const *v, const char *const *names, Op *ops, Grid &g, bool kd5 = false)
 {
     for (int i = 0; i < n; ++i) {
         MCS_REQUIRE(v[i] && v[i]->ptr, "%s: %s is null", fn, names[i]);
-        MCS_REQUIRE(v[i]->sizes[3] == 4, "%s: %s must have 4 channels, got %d", fn, names[i], v[i]->sizes[3]);
+        if (i == 0 && kd5)
+            MCS_REQUIRE(v[i]->sizes[3] == 4 || v[i]->sizes[3] == 5, "%s: %s must have 4 or 5 channels, got %d", fn, names[i], v[i]->sizes[3]);
+        else
+            MCS_REQUIRE(v[i]->sizes[3] == 4, "%s: %s must have 4 channels, got %d", fn, names[i], v[i]->sizes[3]);
         for (int d = 0; d < 3; ++d)
             MCS_REQUIRE(v[i]->sizes[d] == v[0]->sizes[d], "%s: %s must have the shape of %s", fn, names[i], names[0]);
         for (int d = 0; d < 4; ++d) MCS_REQUIRE(v[i]->strides[d] >= 0, "%s: %s has a negative stride", fn, names[i]);
@@ -303,7 +316,8 @@ int views(const char *fn, int n, const mcs_tensor *const *v, const char *const *
         Op &o = ops[i];
         o.p = (const float *)v[i]->ptr;
         o.s0 = st[0]; o.s1 = st[1]; o.s2 = st[2]; o.s3 = st[3];
-        o.vec = ((uintptr_t)o.p & 15) == 0 && st[3] == 1 && (sz[2] == 1 || st[2] == 4) && (sz[1] == 1 || st[1] == 4 * W) &&
+        o.sa = (int64_t)(sz[3] - 1) * st[3];
+        o.vec = sz[3] == 4 && ((uintptr_t)o.p & 15) == 0 && st[3] == 1 && (sz[2] == 1 || st[2] == 4) && (sz[1] == 1 || st[1] == 4 * W) &&
                 (sz[0] == 1 || st[0] == 4 * (int64_t)H * W);
     }
     return 0;
@@ -317,7 +331,7 @@ int reg_fwd(const char *fn, int n, const mcs_tensor *const *v, const char *const
 {
     Op ops[3] = {};
     Grid g{};
-    if (int e = views(fn, n, v, names, ops, g)) return e;
+    if (int e = views(fn, n, v, names, ops, g, FN == FN_SMOOTH)) return e;
     MCS_REQUIRE(partials && loss && (means || FN != FN_SHADING), "%s: null output pointer", fn);
     const cudaStream_t s = (cudaStream_t)stream;
     const int np = npartials(g.npx);
@@ -378,12 +392,13 @@ int mcs_material_smoothness_grad_bwd(const mcs_tensor *kd_grad, const mcs_tensor
     const char *names[3] = {"kd_grad", "ks_grad", "nrm_grad"};
     Op ops[3] = {};
     Grid g{};
-    if (int e = views("material_smoothness_grad_bwd", 3, v, names, ops, g)) return e;
+    if (int e = views("material_smoothness_grad_bwd", 3, v, names, ops, g, true)) return e;
+    const int ckd = kd_grad->sizes[3];
     MCS_REQUIRE(d_loss && d_kd_grad && d_ks_grad && d_nrm_grad, "material_smoothness_grad_bwd: null pointer argument");
-    MCS_REQUIRE(aligned16(d_kd_grad) && aligned16(d_ks_grad) && aligned16(d_nrm_grad),
-                "material_smoothness_grad_bwd: gradient outputs must be 16-byte aligned");
+    MCS_REQUIRE((aligned16(d_kd_grad) || ckd == 5) && aligned16(d_ks_grad) && aligned16(d_nrm_grad),
+                "material_smoothness_grad_bwd: gradient outputs must be 16-byte aligned (d_kd_grad: when 4-channel)");
     k_smooth_bwd<<<(g.npx + RG_THREADS - 1) / RG_THREADS, RG_THREADS, 0, (cudaStream_t)stream>>>(
-        ops[0], ops[1], ops[2], g, Lambdas{lambda_kd, lambda_ks, lambda_nrm}, d_loss, d_kd_grad, d_ks_grad, d_nrm_grad);
+        ops[0], ops[1], ops[2], g, Lambdas{lambda_kd, lambda_ks, lambda_nrm}, ckd, d_loss, d_kd_grad, d_ks_grad, d_nrm_grad);
     MCS_LAUNCH_CHECK();
     return 0;
 }

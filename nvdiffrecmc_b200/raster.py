@@ -8,8 +8,8 @@ those barycentrics and is differentiable with respect to the attributes and to `
 antialiasing of Laine et al. 2020, the only path from coverage (alpha) to vertex positions, so silhouette losses train the mesh;
 `antialias_topology` builds the edge adjacency it needs on the device.  `DepthPeeler` returns the deeper layers of the same G-buffer
 (the next surface along each primary ray), each an ordinary `rast` that `interpolate` and `antialias` take, as render_mesh's
-back-to-front `composite_buffer` needs.  Screen-space derivatives come in nvdiffrast's layout: `rasterize(grad_db=True)` and
-`DepthPeeler(grad_db=True)` also return `rast_db` (du/dX, du/dY, dv/dX, dv/dY in pixels, from the clip-space triangle), and
+back-to-front `composite_buffer` needs; `composite` runs that compositing for every buffer of a layer in one launch each way.
+Screen-space derivatives come in nvdiffrast's layout: `rasterize(grad_db=True)` and `DepthPeeler(grad_db=True)` also return `rast_db` (du/dX, du/dY, dv/dX, dv/dY in pixels, from the clip-space triangle), and
 `interpolate(..., rast_db=, diff_attrs=)` returns the attribute derivatives `out_da` that render_layer turns into the denoiser's depth
 guide (render.py:225-234).  `texture` is nvdiffrast's filtered look-up with its signature, in the modes the reference calls: bilinear
 ('linear') and trilinear on a mip chain with the level of detail taken from `uv_da` ('linear-mipmap-linear', e.g. `gb_texc_deriv`),
@@ -352,6 +352,191 @@ def antialias(color, rast, pos, tri, topology=None):
             raise ValueError("antialias: topology has %d rows for %d triangles" % (topology.shape[0], tri.shape[0]))
     return _antialias_func.apply(color.to(torch.float32).contiguous(), pos.contiguous(), rast.detach().contiguous(), tri.contiguous(),
                                  topology.contiguous())
+
+
+_COMPOSITE_MAX_BUFFERS = 16
+
+
+def _table(views):
+    """ctypes array of mcs_tensor views, one per tensor; None gives a null entry."""
+    arr = (L.mcs_tensor * len(views))()
+    for k, t in enumerate(views):
+        if t is not None:
+            arr[k] = L.nhwc(t)
+    return arr
+
+
+def _packed(slot, shape, cs):
+    """Per-key dense [B,H,W,C_k] accumulators laid end to end in one flat scratch slot."""
+    n = shape[0] * shape[1] * shape[2]
+    offs = [sum(cs[:k]) for k in range(len(cs))]
+    return [slot[n * o:n * (o + c)].view(*shape, c) for o, c in zip(offs, cs)]
+
+
+def _geom_args(rast, pos, tri, topology):
+    return (rast.data_ptr(), *_pos_args(pos), tri.data_ptr(), tri.shape[0], topology.data_ptr())
+
+
+def _composite_layers(rasts, bgs, bufs, pos, tri, topology, keep):
+    """The forward launches, back to front.  bufs[l] is layer l's list of buffers, bgs one background or None per key.  Returns the per-key
+    outputs and the scratch: with keep, slot l holds layer l's input accumulator for l < nl - 1 (the deepest layer's is bgs); without
+    keep the accumulators between layers ping-pong in two slots."""
+    n, nl = len(bgs), len(rasts)
+    shape = tuple(rasts[0].shape[:3])
+    cs = [t.shape[3] for t in bufs[0]]
+    dev = rasts[0].device
+    outs = [torch.empty(*shape, c, dtype=torch.float32, device=dev) for c in cs]
+    slots = nl - 1 if keep else min(nl - 1, 2)
+    scratch = torch.empty(slots, shape[0] * shape[1] * shape[2] * sum(cs), dtype=torch.float32, device=dev) if slots else None
+    for l in reversed(range(nl)):
+        acc_in = bgs if l == nl - 1 else _packed(scratch[l if keep else (l + 1) % slots], shape, cs)
+        acc_out = outs if l == 0 else _packed(scratch[l - 1 if keep else l % slots], shape, cs)
+        L.check(L.lib().mcs_composite_fwd(n, _table(bufs[l]), _table(acc_in), _table(acc_out), *_geom_args(rasts[l], pos, tri, topology),
+                                          L.stream_ptr()), "composite_fwd")
+    return outs, scratch
+
+
+class _composite_func(torch.autograd.Function):
+    """inputs: buffer count n, layer count nl, pos, tri, topology, then the nl rasts, the n backgrounds (None where absent) and the
+    nl * n buffers, layer-major.  One launch per layer each way."""
+    @staticmethod
+    def forward(ctx, n, nl, pos, tri, topology, *flat):
+        rasts, bgs = flat[:nl], flat[nl:nl + n]
+        bufs = [flat[nl + n + l * n:nl + n + (l + 1) * n] for l in range(nl)]
+        outs, scratch = _composite_layers(rasts, bgs, bufs, pos, tri, topology, keep=True)
+        ctx.n, ctx.nl = n, nl
+        ctx.save_for_backward(pos, tri, topology, scratch, *flat)
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *d_outs):
+        n, nl = ctx.n, ctx.nl
+        pos, tri, topology, scratch, *flat = ctx.saved_tensors
+        rasts, bgs = flat[:nl], flat[nl:nl + n]
+        bufs = [flat[nl + n + l * n:nl + n + (l + 1) * n] for l in range(nl)]
+        need = ctx.needs_input_grad
+        need_pos, need_bg, need_buf = need[2], need[5 + nl:5 + nl + n], need[5 + nl + n:]
+        shape = tuple(rasts[0].shape[:3])
+        cs = [t.shape[3] for t in bufs[0]]
+        dev = rasts[0].device
+        new = lambda c: torch.empty(*shape, c, dtype=torch.float32, device=dev)
+        d_pos = torch.zeros_like(pos) if need_pos else None
+        d_bgs = [new(c) if need_bg[k] else None for k, c in enumerate(cs)]
+        d_bufs = [[new(c) if need_buf[l * n + k] else None for k, c in enumerate(cs)] for l in range(nl)]
+        slots = min(nl - 1, 2)
+        gp = torch.empty(slots, shape[0] * shape[1] * shape[2] * sum(cs), dtype=torch.float32, device=dev) if slots else None
+        g = [d.to(torch.float32) for d in d_outs]
+        for l in range(nl):
+            acc_in = bgs if l == nl - 1 else _packed(scratch[l], shape, cs)
+            d_in = d_bgs if l == nl - 1 else _packed(gp[l % slots], shape, cs)
+            L.check(L.lib().mcs_composite_bwd(n, _table(bufs[l]), _table(acc_in), _table(g), _table(d_in), _table(d_bufs[l]),
+                                              *_geom_args(rasts[l], pos, tri, topology), d_pos.data_ptr() if d_pos is not None else None,
+                                              L.stream_ptr()), "composite_bwd")
+            g = d_in
+        return (None, None, d_pos, None, None, *([None] * nl), *d_bgs, *[d for ds in d_bufs for d in ds])
+
+
+def _composite_args(layers, pos, tri, background, topology):
+    """Validated (keys, rasts, per-layer buffer lists, per-key backgrounds, pos, tri, topology); ValueError naming the argument."""
+    fn = "composite"
+
+    def check(what, t, dev, dtype=torch.float32):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError("%s: %s must be a torch.Tensor, got %s" % (fn, what, type(t).__name__))
+        if t.dtype != dtype:
+            raise ValueError("%s: %s must be %s, got %s" % (fn, what, str(dtype).replace("torch.", ""), t.dtype))
+        if not t.is_cuda:
+            raise ValueError("%s: %s must be a CUDA tensor, got %s" % (fn, what, t.device))
+        if dev is not None and t.device != dev:
+            raise ValueError("%s: %s is on %s, layers[0]'s rast on %s" % (fn, what, t.device, dev))
+        if any(s >= 2 ** 31 for s in t.stride()):
+            raise ValueError("%s: %s has a stride beyond int32" % (fn, what))
+
+    if not isinstance(layers, (list, tuple)) or not layers:
+        raise ValueError("%s: layers must be a non-empty list of (buffers, rast[, rast_db]) tuples" % fn)
+    for l, layer in enumerate(layers):
+        if not isinstance(layer, (list, tuple)) or len(layer) not in (2, 3) or not isinstance(layer[0], dict):
+            raise ValueError("%s: layers[%d] must be a (buffers dict, rast[, rast_db]) tuple" % (fn, l))
+    keys = list(layers[0][0].keys())
+    if not keys or len(keys) > _COMPOSITE_MAX_BUFFERS:
+        raise ValueError("%s: layers hold %d buffers; 1 to %d are supported" % (fn, len(keys), _COMPOSITE_MAX_BUFFERS))
+    check("layers[0]'s rast", layers[0][1], None)
+    dev = layers[0][1].device
+    shape = tuple(layers[0][1].shape)
+    if len(shape) != 4 or shape[3] != 4 or 0 in shape:
+        raise ValueError("%s: layers[0]'s rast must be a non-empty [B,H,W,4], got %s" % (fn, shape))
+    B, H, W = shape[:3]
+    cs = {}
+    rasts, bufs = [], []
+    for l, (buffers, rast, *_) in enumerate(layers):
+        if set(buffers) != set(keys):
+            raise ValueError("%s: layers[%d] has the keys %s, layers[0] %s" % (fn, l, sorted(buffers), sorted(keys)))
+        check("layers[%d]'s rast" % l, rast, dev)
+        if tuple(rast.shape) != shape:
+            raise ValueError("%s: layers[%d]'s rast is %s, layers[0]'s %s" % (fn, l, tuple(rast.shape), shape))
+        for k in keys:
+            t = buffers[k]
+            what = "layers[%d][%r]" % (l, k)
+            check(what, t, dev)
+            if t.dim() != 4 or tuple(t.shape[:3]) != (B, H, W) or t.shape[3] < 1:
+                raise ValueError("%s: %s must be [%d,%d,%d,C] with C >= 1 like rast, got %s" % (fn, what, B, H, W, tuple(t.shape)))
+            if cs.setdefault(k, t.shape[3]) != t.shape[3]:
+                raise ValueError("%s: %s has %d channels, layers[0][%r] %d" % (fn, what, t.shape[3], k, cs[k]))
+        rasts.append(rast.detach().contiguous())
+        bufs.append([buffers[k] for k in keys])
+    if H * W * sum(cs.values()) >= 2 ** 31:
+        raise ValueError("%s: layers: H * W * (sum of the channels) must stay below 2^31" % fn)
+    check("pos", pos, dev)
+    if not (pos.dim() == 2 and pos.shape[1] == 4) and not (pos.dim() == 3 and pos.shape[2] == 4 and pos.shape[0] == B) or pos.shape[-2] == 0:
+        raise ValueError("%s: pos must be [V,4] or [%d,V,4], got %s" % (fn, B, tuple(pos.shape)))
+    check("tri", tri, dev, torch.int32)
+    if tri.dim() != 2 or tri.shape[1] != 3 or tri.shape[0] == 0:
+        raise ValueError("%s: tri must be a non-empty [T,3], got %s" % (fn, tuple(tri.shape)))
+    bgs = [None] * len(keys)
+    if background is not None:
+        if not isinstance(background, dict):
+            raise ValueError("%s: background must be a dict from buffer key to accumulator, got %s" % (fn, type(background).__name__))
+        for k, t in background.items():
+            if k not in cs:
+                raise ValueError("%s: background key %r is not a buffer key" % (fn, k))
+            what = "background[%r]" % (k,)
+            check(what, t, dev)
+            if tuple(t.shape) != (B, H, W, cs[k]):
+                raise ValueError("%s: %s must be [%d,%d,%d,%d], got %s" % (fn, what, B, H, W, cs[k], tuple(t.shape)))
+            bgs[keys.index(k)] = t
+    if topology is not None:
+        check("topology", topology, dev, torch.int32)
+        if topology.dim() != 2 or topology.shape[1] != 3 or topology.shape[0] != tri.shape[0]:
+            raise ValueError("%s: topology must be [T,3] with T = %d like tri, got %s" % (fn, tri.shape[0], tuple(topology.shape)))
+    return keys, rasts, bufs, bgs, pos.contiguous(), tri.contiguous(), topology
+
+
+def composite(layers, pos, tri, background=None, topology=None):
+    """render_mesh's compositing (the reference's composite_buffer with antialias, render/render.py:284-291, run for every key at
+    :321-330), every buffer of a layer in one launch each way.
+
+    layers: render_mesh's list, front to back, of (buffers, rast[, rast_db]) with buffers a dict of fp32 CUDA [B,H,W,C_k] tensors (any
+    strides, C_k >= 1, the same keys and channel counts in every layer, at most 16) and rast that layer's [B,H,W,4] (rast_db is ignored).
+    pos the clip-space vertices [V,4] or [B,V,4] and tri int32 [T,3] the layers were rasterised from, as for `antialias`.  background: a
+    dict from key to that key's full [B,H,W,C_k] starting accumulator, e.g. render_mesh's cat((background, zeros)) for 'shaded'; a key
+    without one starts from zeros.  topology: `antialias_topology(tri)`, built inside the call when None.
+
+    Returns {key: accumulator} for every key: back to front, alpha = (rast.w > 0) * buf[..., -1], accum = antialias(lerp(accum,
+    (buf[..., :-1], 1), alpha)), bit for bit what that torch chain computes with `antialias`.  Differentiable in every buffer (alpha
+    included), in pos and in background.  No host sync; capturable in a CUDA graph when topology is given.  Malformed input raises
+    ValueError naming the argument before any launch.  Semantics: csrc/composite.cu."""
+    keys, rasts, bufs, bgs, pos, tri, topology = _composite_args(layers, pos, tri, background, topology)
+    if topology is None:
+        topology = antialias_topology(tri)
+    topology = topology.contiguous()
+    flat = [*rasts, *bgs, *[t for ts in bufs for t in ts]]
+    if torch.is_grad_enabled() and (pos.requires_grad or any(t is not None and t.requires_grad for t in flat)):
+        outs = _composite_func.apply(len(keys), len(rasts), pos, tri, topology, *flat)
+    else:
+        det = lambda t: None if t is None else t.detach()
+        outs, _ = _composite_layers(rasts, [det(t) for t in bgs], [[t.detach() for t in ts] for ts in bufs], pos.detach(), tri, topology,
+                                    keep=False)
+    return dict(zip(keys, outs))
 
 
 _TEX_FILTERS = {"linear": 0, "linear-mipmap-linear": 1}

@@ -8,7 +8,8 @@ each (plus a one-CTA finish in the forward), make no host synchronisation and ca
 upstream gradient from the device.  Gradients flow to every rendered operand, all four channels (alpha comes from the composite and
 depends on the geometry); `kd`'s alpha gets exactly 0 and `color_ref` is the constant target.
 
-Operands are fp32 CUDA [B,H,W,4] tensors of one shape, with any strides (`color_ref` is often a slice).  A wrong channel count, a shape
+Operands are fp32 CUDA [B,H,W,4] tensors of one B, H, W, with any strides (`color_ref` is often a slice); `material_smoothness_grad`'s
+kd_grad may also be [B,H,W,5], the transparency configuration's 4-channel kd with alpha appended.  A wrong channel count, a shape
 mismatch, a CPU tensor, a non-float lambda or a `color_ref` that requires grad raises ValueError before anything is launched.
 """
 import torch
@@ -18,20 +19,22 @@ from . import _lib as L
 __all__ = ["shading_loss", "material_smoothness_grad", "chroma_loss", "jitter_taps"]
 
 
-def _check(fn, named, lambdas):
-    """ValueError naming the argument unless every (name, tensor) of `named` is an fp32 CUDA [B,H,W,4] tensor of the first one's shape on
-    its device, every (name, value) of `lambdas` is a Python float, and color_ref (if given) does not require grad."""
+def _check(fn, named, lambdas, chans=None):
+    """ValueError naming the argument unless every (name, tensor) of `named` is an fp32 CUDA [B,H,W,C] tensor of the first one's B, H, W on
+    its device, with C = 4 or one of chans[name], every (name, value) of `lambdas` is a Python float, and color_ref (if given) does not
+    require grad."""
     first_name, first = named[0]
     for name, t in named:
         if not isinstance(t, torch.Tensor):
             raise ValueError("%s: %s must be a torch.Tensor, got %s" % (fn, name, type(t).__name__))
         if t.dtype != torch.float32:
             raise ValueError("%s: %s must be float32, got %s" % (fn, name, t.dtype))
-        if t.dim() != 4 or t.shape[3] != 4:
-            raise ValueError("%s: %s must be [B,H,W,4], got %s" % (fn, name, tuple(t.shape)))
+        want = (chans or {}).get(name, (4,))
+        if t.dim() != 4 or t.shape[3] not in want:
+            raise ValueError("%s: %s must be [B,H,W,%s], got %s" % (fn, name, "|".join(map(str, want)), tuple(t.shape)))
         if not t.is_cuda:
             raise ValueError("%s: %s must be a CUDA tensor, got %s" % (fn, name, t.device))
-        if t.shape != first.shape:
+        if t.shape[:3] != first.shape[:3]:
             raise ValueError("%s: %s has shape %s, %s has %s" % (fn, name, tuple(t.shape), first_name, tuple(first.shape)))
         if t.device != first.device:
             raise ValueError("%s: %s is on %s, %s on %s" % (fn, name, t.device, first_name, first.device))
@@ -124,9 +127,10 @@ class _MaterialSmoothness(torch.autograd.Function):
 
 def material_smoothness_grad(kd_grad, ks_grad, nrm_grad, lambda_kd=0.25, lambda_ks=0.1, lambda_nrm=0.0):
     """The reference's material smoothness regulariser over the jittered-tap differences kd_grad, ks_grad, nrm_grad (rgb, coverage
-    alpha).  -> 0-dim fp32 tensor, differentiable in all four channels of each."""
+    alpha).  kd_grad may have 5 channels (`jitter_taps` of a 4-channel kd): luma from channels 0..2, alpha from the last, and channel 3
+    gets a gradient of exactly 0.  -> 0-dim fp32 tensor, differentiable in every channel of each."""
     _check("material_smoothness_grad", [("kd_grad", kd_grad), ("ks_grad", ks_grad), ("nrm_grad", nrm_grad)],
-           [("lambda_kd", lambda_kd), ("lambda_ks", lambda_ks), ("lambda_nrm", lambda_nrm)])
+           [("lambda_kd", lambda_kd), ("lambda_ks", lambda_ks), ("lambda_nrm", lambda_nrm)], chans={"kd_grad": (4, 5)})
     if torch.is_grad_enabled() and (kd_grad.requires_grad or ks_grad.requires_grad or nrm_grad.requires_grad):
         return _MaterialSmoothness.apply(kd_grad, ks_grad, nrm_grad, lambda_kd, lambda_ks, lambda_nrm)
     return _smooth_fwd(kd_grad.detach(), ks_grad.detach(), nrm_grad.detach(), (lambda_kd, lambda_ks, lambda_nrm))

@@ -96,5 +96,17 @@ rb = torch.rand(2, 9, 11, 8, device=dev)
 lights = [torch.rand(2, 9, 11, 4, device=dev, requires_grad=True) for _ in range(2)]
 (reg.shading_loss(*lights, rb[..., 2:6], 0.15, 0.0025) + reg.chroma_loss(lights[0], rb[..., 2:6], 0.025)).backward()
 reg.material_smoothness_grad(torch.rand(2, 9, 11, 8, device=dev)[..., 1:5].requires_grad_(True), lights[0], lights[1], 0.1, 0.05, 0.025).backward()
+# layer compositing: two peeled layers, a 5-channel, a 1-channel and a strided buffer, forward + backward and a no_grad forward
+from nvdiffrecmc_b200.raster import composite
+posc = posg.detach().clone().requires_grad_(True)
+with DepthPeeler(ctx, mg, (24, 24)) as peeler:
+    crs = [peeler.rasterize_next_layer()[0] for _ in range(2)]
+cl = [({"shaded": torch.rand(1, 24, 24, 4, device=dev, requires_grad=True), "kd_grad": torch.rand(1, 24, 24, 5, device=dev, requires_grad=True),
+        "mono": torch.rand(1, 24, 24, 1, device=dev, requires_grad=True), "wide": torch.rand(1, 24, 24, 9, device=dev)[..., 2:6]}, r) for r in crs]
+co = composite(cl, posc, t("tris"), background={"shaded": torch.rand(1, 24, 24, 4, device=dev, requires_grad=True)})
+sum(o.sum() for o in co.values()).backward()
+with torch.no_grad():
+    composite(cl, posc, t("tris"))
+reg.material_smoothness_grad(torch.rand(2, 9, 11, 5, device=dev, requires_grad=True), lights[0], lights[1], 0.1, 0.05, 0.025).backward()
 torch.cuda.synchronize()
 print("sanitize workload ok", float(loss), int(v.sum()), tuple(pts.shape))

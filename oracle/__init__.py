@@ -1,9 +1,10 @@
 """CPU oracle for the nvdiffrecmc hot path -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
 
-numpy/ctypes wrappers around the six C restatements in this directory (see each file's header for what it restates and how it is
+numpy/ctypes wrappers around the nine C restatements in this directory (see each file's header for what it restates and how it is
 pinned): ``Oracle`` and ``Scene`` here wrap ``mcoracle.c``; ``oracle.geometry``, ``oracle.hashgrid``, ``oracle.texture``,
-``oracle.mlptexture`` and ``oracle.dmtet`` wrap the C file of the same name.  Only ``tests/``, ``__graft_entry__.smoke()`` and
-``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import this package; ``nvdiffrecmc_b200`` never does.
+``oracle.mlptexture``, ``oracle.dmtet``, ``oracle.regularizer``, ``oracle.mipchain`` and ``oracle.taps`` wrap the C file of the same
+name.  Only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s ``cpu_baseline`` / ``--impl reference`` legs may import this
+package; ``nvdiffrecmc_b200`` never does.
 
 ``build()`` compiles every library twice from the same source: fp32 (the oracle proper, compared with the CUDA kernels) and fp64
 (``f64=True``), used only to validate derivatives and hand-derived adjoints by finite differences.  ``CLib`` is the wrappers' common base:
@@ -24,7 +25,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _BUILD = os.path.join(_HERE, "_build")
 # library: [its source, then the files that source #includes]
 LIBS = {"mcoracle": ["mcoracle.c", "detmath.h"], "geometry": ["geometry.c"], "hashgrid": ["hashgrid.c"], "texture": ["texture.c"],
-        "mlptexture": ["mlptexture.c", "hashgrid.c"], "dmtet": ["dmtet.c"]}
+        "mlptexture": ["mlptexture.c", "hashgrid.c"], "dmtet": ["dmtet.c"], "regularizer": ["regularizer.c"], "mipchain": ["mipchain.c"],
+        "taps": ["taps.c", "texture.c"]}
 
 
 def _cpu_has_fma():
@@ -96,8 +98,11 @@ class CLib:
             fn = getattr(self.lib, name)          # AttributeError if the library does not export it
             fn.argtypes = [self.real if a is REAL else a for a in args]
             fn.restype = res
-        sizeof_real, = [n for n in self.SIGS if n.endswith("_sizeof_real")]      # every library exports one
-        assert getattr(self.lib, sizeof_real)() == C.sizeof(self.real)
+        # every library exports at least one; one that includes another C file (taps.c: texture.c) also exports that file's
+        sizeof_real = [n for n in self.SIGS if n.endswith("_sizeof_real")]
+        assert sizeof_real, "%s declares no *_sizeof_real" % self.LIB
+        for name in sizeof_real:
+            assert getattr(self.lib, name)() == C.sizeof(self.real), name
 
     @classmethod
     def get(cls, f64=False):

@@ -2,30 +2,17 @@
 
 numpy/ctypes wrapper around ``oracle/mipchain.c``, the restatement of the chain forward, its backward folded over every level, and
 Texture2D's clamp_ / normalize_ (render/texture.py:20-30,89-100; the contract is stated in nvdiffrecmc_b200/csrc/texture.cu).  Two builds
-of the same source: fp32 (``mipchain_oracle()``, compared bit for bit with the kernels) and fp64 (``mipchain_oracle(True)``).  The library
-is built by this module's ``build()`` with the flags of ``oracle.build()``; it is not an entry of ``oracle.LIBS``, whose table the
-signature test of the other libraries pins, so tests/test_oracle_mipchain.py checks this table against the source in the same way.
+of the same source: fp32 (``mipchain_oracle()``, compared bit for bit with the kernels) and fp64 (``mipchain_oracle(True)``).
+``oracle.build()`` compiles both from ``oracle.LIBS``.
 """
 import ctypes as C
 import os
 
 import numpy as np
 
-from oracle import _CFLAGS, _HERE, _I, _P, CLib, _compile, _lib_path
+from oracle import _HERE, _I, _P, LIBS, CLib
 
-LIB = "mipchain"
-SOURCES = ["mipchain.c"]
-
-
-def _build_one(f64, force=False):
-    srcs = [os.path.join(_HERE, s) for s in SOURCES]
-    _compile(["gcc"] + _CFLAGS + (["-DORACLE_F64"] if f64 else []) + [srcs[0], "-lm"], _lib_path(LIB, f64), srcs, force)
-
-
-def build(force=False):
-    """Compile oracle/mipchain.c with gcc, fp32 and fp64 (-DORACLE_F64), into oracle/_build/."""
-    for f64 in (False, True):
-        _build_one(f64, force)
+SOURCES = [os.path.join(_HERE, s) for s in LIBS["mipchain"]]      # path of the library's source
 
 
 def mip_shapes(H, W):
@@ -37,7 +24,7 @@ def mip_shapes(H, W):
 
 
 class MipChainOracle(CLib):
-    LIB = LIB
+    LIB = "mipchain"
     SIGS = {
         "mip_sizeof_real": ([], _I),
         "mip_fwd": ([_I, _I, _I] + [_P] * 3, None),
@@ -45,18 +32,6 @@ class MipChainOracle(CLib):
         "mip_clamp": ([_I, _I, _I] + [_P] * 5, None),
         "mip_normalize": ([_I, _I] + [_P] * 3, None),
     }
-
-    def __init__(self, f64=False):
-        # CLib.__init__ builds from oracle.LIBS; this library builds itself, then loads exactly as CLib does
-        self.f64 = f64
-        self.dt, self.real = (np.float64, C.c_double) if f64 else (np.float32, C.c_float)
-        _build_one(f64)
-        self.lib = C.CDLL(_lib_path(LIB, f64))
-        for name, (args, res) in self.SIGS.items():
-            fn = getattr(self.lib, name)
-            fn.argtypes = args
-            fn.restype = res
-        assert self.lib.mip_sizeof_real() == C.sizeof(self.real)
 
     @staticmethod
     def _table(levels):

@@ -3,34 +3,20 @@
 numpy/ctypes wrapper around ``oracle/regularizer.c``, the restatement of the reference's ``shading_loss``, ``material_smoothness_grad``
 and ``chroma_loss`` (render/regularizer.py:15-49; the contract is stated in nvdiffrecmc_b200/csrc/regularizer.cu).  Two builds of the
 same source: fp32 (``RegularizerOracle.get()``, compared bit for bit with the CUDA gradients of material_smoothness_grad and chroma_loss)
-and fp64 (``RegularizerOracle.get(True)``, checked by finite differences and the per-element bar).  The library is built by this module's
-``build()`` with the flags of ``oracle.build()``; it is not an entry of ``oracle.LIBS``, whose table the signature test of the other
-libraries pins, so tests/test_oracle_regularizer.py checks this table against the source in the same way.
+and fp64 (``RegularizerOracle.get(True)``, checked by finite differences and the per-element bar).  ``oracle.build()`` compiles both
+from ``oracle.LIBS``.
 """
-import ctypes as C
 import os
 
 import numpy as np
 
-from oracle import _CFLAGS, _HERE, _I, _P, REAL, CLib, _compile, _lib_path
+from oracle import _HERE, _I, _P, LIBS, REAL, CLib
 
-LIB = "regularizer"
-SOURCES = ["regularizer.c"]
-
-
-def _build_one(f64, force=False):
-    srcs = [os.path.join(_HERE, s) for s in SOURCES]
-    _compile(["gcc"] + _CFLAGS + (["-DORACLE_F64"] if f64 else []) + [srcs[0], "-lm"], _lib_path(LIB, f64), srcs, force)
-
-
-def build(force=False):
-    """Compile oracle/regularizer.c with gcc, fp32 and fp64 (-DORACLE_F64), into oracle/_build/."""
-    for f64 in (False, True):
-        _build_one(f64, force)
+SOURCES = [os.path.join(_HERE, s) for s in LIBS["regularizer"]]      # path of the library's source
 
 
 class RegularizerOracle(CLib):
-    LIB = LIB
+    LIB = "regularizer"
     SIGS = {
         "reg_sizeof_real": ([], _I),
         "reg_shading_loss_fwd": ([_I] + [_P] * 3 + [REAL, REAL, _P, _P], None),
@@ -40,18 +26,6 @@ class RegularizerOracle(CLib):
         "reg_chroma_loss_fwd": ([_I, _P, _P, REAL, _P], None),
         "reg_chroma_loss_bwd": ([_I, _P, _P, REAL, REAL, _P], None),
     }
-
-    def __init__(self, f64=False):
-        # CLib.__init__ builds from oracle.LIBS; this library builds itself, then loads exactly as CLib does
-        self.f64 = f64
-        self.dt, self.real = (np.float64, C.c_double) if f64 else (np.float32, C.c_float)
-        _build_one(f64)
-        self.lib = C.CDLL(_lib_path(LIB, f64))
-        for name, (args, res) in self.SIGS.items():
-            fn = getattr(self.lib, name)
-            fn.argtypes = [self.real if a is REAL else a for a in args]
-            fn.restype = res
-        assert self.lib.reg_sizeof_real() == C.sizeof(self.real)
 
     def _px4(self, *arrs):
         """[...,4] arrays of one shape -> (leading shape, pixel count, contiguous `real` copies)."""

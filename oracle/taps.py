@@ -4,58 +4,25 @@ numpy/ctypes wrapper around ``oracle/taps.c``, the restatement of shade()'s kd_g
 (render/render.py:50-97; the contract is stated in nvdiffrecmc_b200/csrc/taps.cu), whose tap is texture.c's look-up, included by the C
 file.  Two builds of the same source: fp32 (``taps_oracle()``, compared bit for bit with the kernels' forward and one-writer gradients, and
 per element with their scatters) and fp64 (``taps_oracle(True)``, checked by finite differences and against the reference's own shade()).
-The library is built by this module's ``build()`` with the flags of ``oracle.build()``; like the regulariser and mip-chain oracles it is
-not an entry of ``oracle.LIBS``, whose table the signature test of the other libraries pins, so tests/test_oracle_taps.py checks this
-table against the source in the same way.
+``oracle.build()`` compiles both from ``oracle.LIBS``.  The library also exports texture.c's functions, so ``TapsOracle.SIGS`` extends
+``TextureOracle.SIGS``.
 """
-import ctypes as C
-import os
-
 import numpy as np
 
-from oracle import _CFLAGS, _HERE, _I, _P, TERMS, CLib, _compile, _lib_path
+from oracle import _I, _P, TERMS, CLib
+from oracle.texture import TextureOracle
 
-LIB = "taps"
-SOURCES = ["taps.c", "texture.c"]
 BUFFERS = ["kd_grad", "ks_grad", "normal_grad", "perturbed_nrm_grad"]
 OPERANDS = ["kd", "ks", "gb_normal", "perturbed_nrm", "kd_jitter", "ks_jitter"]
 
 
-def _build_one(f64, force=False):
-    srcs = [os.path.join(_HERE, s) for s in SOURCES]
-    _compile(["gcc"] + _CFLAGS + (["-DORACLE_F64"] if f64 else []) + [srcs[0], "-lm"], _lib_path(LIB, f64), srcs, force)
-
-
-def build(force=False):
-    """Compile oracle/taps.c (with the texture.c it includes) with gcc, fp32 and fp64 (-DORACLE_F64), into oracle/_build/."""
-    for f64 in (False, True):
-        _build_one(f64, force)
-
-
 class TapsOracle(CLib):
-    LIB = LIB
-    SIGS = {
+    LIB = "taps"
+    SIGS = dict(TextureOracle.SIGS, **{
         "taps_sizeof_real": ([], _I),
         "taps_fwd": ([_I] * 4 + [_P] * 12, None),
         "taps_bwd": ([_I] * 4 + [_P] * 18 + [_I], None),
-        # texture.c, included by taps.c
-        "tex_sizeof_real": ([], _I),
-        "tex_log2f": ([C.c_float], C.c_float),
-        "tex_fwd": ([_I, _I] + [_P] * 6 + [_I] * 5 + [_P], None),
-        "tex_bwd": ([_I, _I] + [_P] * 6 + [_I] * 5 + [_P] * 4 + [_I], None),
-    }
-
-    def __init__(self, f64=False):
-        # CLib.__init__ builds from oracle.LIBS; this library builds itself, then loads exactly as CLib does
-        self.f64 = f64
-        self.dt, self.real = (np.float64, C.c_double) if f64 else (np.float32, C.c_float)
-        _build_one(f64)
-        self.lib = C.CDLL(_lib_path(LIB, f64))
-        for name, (args, res) in self.SIGS.items():
-            fn = getattr(self.lib, name)
-            fn.argtypes = args
-            fn.restype = res
-        assert self.lib.taps_sizeof_real() == C.sizeof(self.real)
+    })
 
     def _ops(self, rast, jitter, kd, ks, gb_normal, perturbed_nrm, kd_jitter, ks_jitter):
         B, H, W = np.shape(rast)[:3]

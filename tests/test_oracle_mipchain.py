@@ -4,7 +4,6 @@ points of the chain."""
 import ctypes
 import importlib
 import os
-import re
 import sys
 
 import numpy as np
@@ -12,7 +11,7 @@ import pytest
 import torch
 
 from common import rel_l2
-from oracle.mipchain import MipChainOracle, mip_shapes, mipchain_oracle
+from oracle.mipchain import mip_shapes, mipchain_oracle
 from nvdiffrecmc_b200 import _lib
 
 REF = "/root/reference/render/texture.py"
@@ -143,21 +142,6 @@ def test_normalize_is_safe_normalize():
         assert g[~fin & ~np.isnan(g)].tobytes() == ref[~fin & ~np.isnan(ref)].tobytes()
     small = np.float32(1e-12) / np.sqrt(np.float32(1e-20))              # below eps the length is sqrt(1e-20)
     assert same_bits(got[1][0, 0, :4], np.array([[0, 0, 0], [small, 0, 0], [0.6, 0.8, 0], [-0.0, 0, 1]], np.float32))
-
-
-def test_signature_table_names_exactly_the_exports():
-    """Every mip_* function oracle/mipchain.c defines has a declared signature, and every declared signature names one (the check
-    tests/test_oracle_signatures.py makes for the libraries of oracle.LIBS)."""
-    import oracle.mipchain
-    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(os.path.dirname(oracle.mipchain.__file__), oracle.mipchain.SOURCES[0])).read(), flags=re.S)
-    names = sorted(re.findall(r"^(?!static\b)[A-Za-z_][\w \*]*?\b(mip_\w+)\s*\([^;{]*\)\s*\{", src, re.M))
-    assert len(names) == 5 and sorted(MipChainOracle.SIGS) == names
-    for f64 in (False, True):
-        o = MipChainOracle.get(f64)
-        assert o is MipChainOracle.get(f64) and o.f64 == f64
-        for name, (args, res) in MipChainOracle.SIGS.items():
-            fn = getattr(o.lib, name)
-            assert fn.restype is res and list(fn.argtypes) == args, name
 
 
 # ---- the C entry points refuse bad tables before any launch ------------------------------------------------------------------------

@@ -10,21 +10,25 @@ from oracle import LIBS, REAL, Oracle
 from oracle.dmtet import DmtetOracle
 from oracle.geometry import GeometryOracle
 from oracle.hashgrid import HashGridOracle
+from oracle.mipchain import MipChainOracle
 from oracle.mlptexture import MlpTextureOracle
+from oracle.regularizer import RegularizerOracle
+from oracle.taps import TapsOracle
 from oracle.texture import TextureOracle
 
 ORACLE_DIR = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
 WRAPPERS = [(Oracle, 48), (GeometryOracle, 15), (HashGridOracle, 4), (TextureOracle, 4), (MlpTextureOracle, 7),
-            (DmtetOracle, 9)]     # exports of each library at the time of writing
+            (DmtetOracle, 9), (RegularizerOracle, 7), (MipChainOracle, 5), (TapsOracle, 7)]     # exports of each library at the time of writing
 
 
 def _exports(lib):
-    """Names of the non-static orc_* / geo_* / hg_* / tex_* / mlt_* / dmt_* function definitions of every C file of a library."""
+    """Names of the non-static orc_* / geo_* / hg_* / tex_* / mlt_* / dmt_* / reg_* / mip_* / taps_* function definitions of every C file
+    of a library."""
     names = []
     for source in LIBS[lib]:
         if source.endswith(".c"):
             src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ORACLE_DIR, source)).read(), flags=re.S)
-            names += re.findall(r"^(?!static\b)[A-Za-z_][\w \*]*?\b((?:orc|geo|hg|tex|mlt|dmt)_\w+)\s*\([^;{]*\)\s*\{", src, re.M)
+            names += re.findall(r"^(?!static\b)[A-Za-z_][\w \*]*?\b((?:orc|geo|hg|tex|mlt|dmt|reg|mip|taps)_\w+)\s*\([^;{]*\)\s*\{", src, re.M)
     return sorted(names)
 
 

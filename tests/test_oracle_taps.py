@@ -2,13 +2,12 @@
 tests/golden/ref_jitter_taps.npz, against central finite differences in fp64, and the argument checks of `jitter_taps` that run before
 any launch."""
 import os
-import re
 
 import numpy as np
 import pytest
 import torch
 
-from oracle.taps import BUFFERS, TapsOracle, taps_oracle
+from oracle.taps import BUFFERS, taps_oracle
 from taps_cases import ARGS, random_case
 from nvdiffrecmc_b200 import _lib
 from nvdiffrecmc_b200.regularizer import jitter_taps
@@ -92,23 +91,6 @@ def test_terms_modes():
         assert np.all(a[k] >= np.abs(s[k]) * (1 - 1e-5)), k
         assert np.all(n[k] == np.round(n[k])) and n[k].max() >= 2, k
     assert n["kd"][..., 3].max() >= 5
-
-
-def test_signature_table_names_exactly_the_exports():
-    """Every function oracle/taps.c and the texture.c it includes define has a declared signature, and every declared signature names
-    one (the check tests/test_oracle_signatures.py makes for the libraries of oracle.LIBS)."""
-    here = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle")
-    names = []
-    for f in ("taps.c", "texture.c"):
-        with open(os.path.join(here, f)) as fh:
-            names += re.findall(r"^(?!static\b)[A-Za-z_][\w \*]*?\b((?:taps|tex)_\w+)\s*\([^;{]*\)\s*\{", fh.read(), re.M)
-    assert sorted(TapsOracle.SIGS) == sorted(names)
-    for f64 in (False, True):
-        o = TapsOracle.get(f64)
-        assert o is TapsOracle.get(f64) and o.f64 == f64
-        for name, (args, res) in TapsOracle.SIGS.items():
-            fn = getattr(o.lib, name)
-            assert fn.restype is res and list(fn.argtypes) == args, name
 
 
 def test_header_declares_both_entry_points():

@@ -293,6 +293,18 @@ int mcs_composite_fwd(int32_t n_buffers, const mcs_tensor *buffers, const mcs_te
 int mcs_composite_bwd(int32_t n_buffers, const mcs_tensor *buffers, const mcs_tensor *accum_in, const mcs_tensor *d_accum_out,
                       const mcs_tensor *d_accum_in, const mcs_tensor *d_buffers, const float *rast, const float *pos, int64_t pos_batch_stride,
                       int32_t V, const int32_t *tris, int32_t T, const int32_t *adj, float *d_pos, mcs_stream stream);
+/*      Supersampled (render_mesh with spp > 1): rast is [B,H,W,4] at full resolution, B, H, W and spp (>= 1, dividing H and W) given
+ *      explicitly.  Each table is at full resolution [B,H,W,C_k] or at output resolution [B,H/spp,W/spp,C_k], the same for every entry of
+ *      the table; d_buffers at the resolution of buffers, d_accum_in at that of accum_in.  An output-resolution input is read nearest
+ *      (pixel (y, x) reads (y / spp, x / spp)); an output-resolution accum_out is the spp x spp box filter of the full-resolution result
+ *      (avg_pool2d), and d_accum_out there the gradient of that filtered output.  With spp = 1 these are mcs_composite_fwd / _bwd. */
+int mcs_composite_ss_fwd(int32_t n_buffers, const mcs_tensor *buffers, const mcs_tensor *accum_in, const mcs_tensor *accum_out, int32_t B,
+                         int32_t H, int32_t W, int32_t spp, const float *rast, const float *pos, int64_t pos_batch_stride, int32_t V,
+                         const int32_t *tris, int32_t T, const int32_t *adj, mcs_stream stream);
+int mcs_composite_ss_bwd(int32_t n_buffers, const mcs_tensor *buffers, const mcs_tensor *accum_in, const mcs_tensor *d_accum_out,
+                         const mcs_tensor *d_accum_in, const mcs_tensor *d_buffers, int32_t B, int32_t H, int32_t W, int32_t spp, const float *rast,
+                         const float *pos, int64_t pos_batch_stride, int32_t V, const int32_t *tris, int32_t T, const int32_t *adj, float *d_pos,
+                         mcs_stream stream);
 
 int mcs_texel_fetch_fwd(const float *tex, int64_t T, int32_t C, const int64_t *idx, int64_t n, float *out, mcs_stream stream);
 int mcs_texel_fetch_bwd(int64_t T, int32_t C, const int64_t *idx, int64_t n, const float *d_out, float *d_tex, mcs_stream stream);

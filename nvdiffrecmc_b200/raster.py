@@ -8,7 +8,8 @@ those barycentrics and is differentiable with respect to the attributes and to `
 antialiasing of Laine et al. 2020, the only path from coverage (alpha) to vertex positions, so silhouette losses train the mesh;
 `antialias_topology` builds the edge adjacency it needs on the device.  `DepthPeeler` returns the deeper layers of the same G-buffer
 (the next surface along each primary ray), each an ordinary `rast` that `interpolate` and `antialias` take, as render_mesh's
-back-to-front `composite_buffer` needs; `composite` runs that compositing for every buffer of a layer in one launch each way.
+back-to-front `composite_buffer` needs; `composite` runs that compositing for every buffer of a layer in one launch each way, and with
+spp > 1 reads MSAA-shaded buffers nearest and box-filters the result as render_mesh does.
 Screen-space derivatives come in nvdiffrast's layout: `rasterize(grad_db=True)` and `DepthPeeler(grad_db=True)` also return `rast_db` (du/dX, du/dY, dv/dX, dv/dY in pixels, from the clip-space triangle), and
 `interpolate(..., rast_db=, diff_attrs=)` returns the attribute derivatives `out_da` that render_layer turns into the denoiser's depth
 guide (render.py:225-234).  `texture` is nvdiffrast's filtered look-up with its signature, in the modes the reference calls: bilinear
@@ -16,6 +17,7 @@ guide (render.py:225-234).  `texture` is nvdiffrast's filtered look-up with its 
 'wrap' or 'clamp' borders, differentiable with respect to the texture, every mip level, uv and uv_da (Texture2D.sample, texture.py:57-68,
 its mip chain's backward and the regulariser taps of render.py)."""
 import ctypes
+import numbers
 
 import torch
 from . import _lib as L
@@ -377,67 +379,68 @@ def _geom_args(rast, pos, tri, topology):
     return (rast.data_ptr(), *_pos_args(pos), tri.data_ptr(), tri.shape[0], topology.data_ptr())
 
 
-def _composite_layers(rasts, bgs, bufs, pos, tri, topology, keep):
+def _composite_layers(rasts, bgs, bufs, pos, tri, topology, spp, keep):
     """The forward launches, back to front.  bufs[l] is layer l's list of buffers, bgs one background or None per key.  Returns the per-key
-    outputs and the scratch: with keep, slot l holds layer l's input accumulator for l < nl - 1 (the deepest layer's is bgs); without
-    keep the accumulators between layers ping-pong in two slots."""
+    outputs (at output resolution, resolved by the front layer) and the scratch of full-resolution accumulators: with keep, slot l holds
+    layer l's input accumulator for l < nl - 1 (the deepest layer's is bgs); without keep the accumulators between layers ping-pong in two
+    slots."""
     n, nl = len(bgs), len(rasts)
-    shape = tuple(rasts[0].shape[:3])
+    B, H, W = shape = tuple(rasts[0].shape[:3])
     cs = [t.shape[3] for t in bufs[0]]
     dev = rasts[0].device
-    outs = [torch.empty(*shape, c, dtype=torch.float32, device=dev) for c in cs]
+    outs = [torch.empty(B, H // spp, W // spp, c, dtype=torch.float32, device=dev) for c in cs]
     slots = nl - 1 if keep else min(nl - 1, 2)
-    scratch = torch.empty(slots, shape[0] * shape[1] * shape[2] * sum(cs), dtype=torch.float32, device=dev) if slots else None
+    scratch = torch.empty(slots, B * H * W * sum(cs), dtype=torch.float32, device=dev) if slots else None
     for l in reversed(range(nl)):
         acc_in = bgs if l == nl - 1 else _packed(scratch[l if keep else (l + 1) % slots], shape, cs)
         acc_out = outs if l == 0 else _packed(scratch[l - 1 if keep else l % slots], shape, cs)
-        L.check(L.lib().mcs_composite_fwd(n, _table(bufs[l]), _table(acc_in), _table(acc_out), *_geom_args(rasts[l], pos, tri, topology),
-                                          L.stream_ptr()), "composite_fwd")
+        L.check(L.lib().mcs_composite_ss_fwd(n, _table(bufs[l]), _table(acc_in), _table(acc_out), B, H, W, spp,
+                                             *_geom_args(rasts[l], pos, tri, topology), L.stream_ptr()), "composite_fwd")
     return outs, scratch
 
 
 class _composite_func(torch.autograd.Function):
-    """inputs: buffer count n, layer count nl, pos, tri, topology, then the nl rasts, the n backgrounds (None where absent) and the
+    """inputs: buffer count n, layer count nl, spp, pos, tri, topology, then the nl rasts, the n backgrounds (None where absent) and the
     nl * n buffers, layer-major.  One launch per layer each way."""
     @staticmethod
-    def forward(ctx, n, nl, pos, tri, topology, *flat):
+    def forward(ctx, n, nl, spp, pos, tri, topology, *flat):
         rasts, bgs = flat[:nl], flat[nl:nl + n]
         bufs = [flat[nl + n + l * n:nl + n + (l + 1) * n] for l in range(nl)]
-        outs, scratch = _composite_layers(rasts, bgs, bufs, pos, tri, topology, keep=True)
-        ctx.n, ctx.nl = n, nl
+        outs, scratch = _composite_layers(rasts, bgs, bufs, pos, tri, topology, spp, keep=True)
+        ctx.n, ctx.nl, ctx.spp = n, nl, spp
         ctx.save_for_backward(pos, tri, topology, scratch, *flat)
         return tuple(outs)
 
     @staticmethod
     def backward(ctx, *d_outs):
-        n, nl = ctx.n, ctx.nl
+        n, nl, spp = ctx.n, ctx.nl, ctx.spp
         pos, tri, topology, scratch, *flat = ctx.saved_tensors
         rasts, bgs = flat[:nl], flat[nl:nl + n]
         bufs = [flat[nl + n + l * n:nl + n + (l + 1) * n] for l in range(nl)]
         need = ctx.needs_input_grad
-        need_pos, need_bg, need_buf = need[2], need[5 + nl:5 + nl + n], need[5 + nl + n:]
-        shape = tuple(rasts[0].shape[:3])
+        need_pos, need_bg, need_buf = need[3], need[6 + nl:6 + nl + n], need[6 + nl + n:]
+        B, H, W = shape = tuple(rasts[0].shape[:3])
         cs = [t.shape[3] for t in bufs[0]]
         dev = rasts[0].device
-        new = lambda c: torch.empty(*shape, c, dtype=torch.float32, device=dev)
+        new = lambda t: torch.empty(t.shape, dtype=torch.float32, device=dev)
         d_pos = torch.zeros_like(pos) if need_pos else None
-        d_bgs = [new(c) if need_bg[k] else None for k, c in enumerate(cs)]
-        d_bufs = [[new(c) if need_buf[l * n + k] else None for k, c in enumerate(cs)] for l in range(nl)]
+        d_bgs = [new(bgs[k]) if need_bg[k] else None for k in range(n)]
+        d_bufs = [[new(t) if need_buf[l * n + k] else None for k, t in enumerate(bufs[l])] for l in range(nl)]
         slots = min(nl - 1, 2)
-        gp = torch.empty(slots, shape[0] * shape[1] * shape[2] * sum(cs), dtype=torch.float32, device=dev) if slots else None
+        gp = torch.empty(slots, B * H * W * sum(cs), dtype=torch.float32, device=dev) if slots else None
         g = [d.to(torch.float32) for d in d_outs]
         for l in range(nl):
             acc_in = bgs if l == nl - 1 else _packed(scratch[l], shape, cs)
             d_in = d_bgs if l == nl - 1 else _packed(gp[l % slots], shape, cs)
-            L.check(L.lib().mcs_composite_bwd(n, _table(bufs[l]), _table(acc_in), _table(g), _table(d_in), _table(d_bufs[l]),
-                                              *_geom_args(rasts[l], pos, tri, topology), d_pos.data_ptr() if d_pos is not None else None,
-                                              L.stream_ptr()), "composite_bwd")
+            L.check(L.lib().mcs_composite_ss_bwd(n, _table(bufs[l]), _table(acc_in), _table(g), _table(d_in), _table(d_bufs[l]), B, H, W, spp,
+                                                 *_geom_args(rasts[l], pos, tri, topology), d_pos.data_ptr() if d_pos is not None else None,
+                                                 L.stream_ptr()), "composite_bwd")
             g = d_in
-        return (None, None, d_pos, None, None, *([None] * nl), *d_bgs, *[d for ds in d_bufs for d in ds])
+        return (None, None, None, d_pos, None, None, *([None] * nl), *d_bgs, *[d for ds in d_bufs for d in ds])
 
 
-def _composite_args(layers, pos, tri, background, topology):
-    """Validated (keys, rasts, per-layer buffer lists, per-key backgrounds, pos, tri, topology); ValueError naming the argument."""
+def _composite_args(layers, pos, tri, background, topology, spp):
+    """Validated (keys, rasts, per-layer buffer lists, per-key backgrounds, pos, tri, topology, spp); ValueError naming the argument."""
     fn = "composite"
 
     def check(what, t, dev, dtype=torch.float32):
@@ -452,6 +455,9 @@ def _composite_args(layers, pos, tri, background, topology):
         if any(s >= 2 ** 31 for s in t.stride()):
             raise ValueError("%s: %s has a stride beyond int32" % (fn, what))
 
+    if isinstance(spp, bool) or not isinstance(spp, numbers.Integral) or spp < 1:
+        raise ValueError("%s: spp must be an integer >= 1, got %r" % (fn, spp))
+    spp = int(spp)
     if not isinstance(layers, (list, tuple)) or not layers:
         raise ValueError("%s: layers must be a non-empty list of (buffers, rast[, rast_db]) tuples" % fn)
     for l, layer in enumerate(layers):
@@ -466,7 +472,11 @@ def _composite_args(layers, pos, tri, background, topology):
     if len(shape) != 4 or shape[3] != 4 or 0 in shape:
         raise ValueError("%s: layers[0]'s rast must be a non-empty [B,H,W,4], got %s" % (fn, shape))
     B, H, W = shape[:3]
+    if H % spp or W % spp:
+        raise ValueError("%s: spp %d does not divide H x W = %d x %d of layers[0]'s rast" % (fn, spp, H, W))
+    Ho, Wo = H // spp, W // spp
     cs = {}
+    res = None                                       # the buffers' resolution, (H, W) or (Ho, Wo), set by the first buffer
     rasts, bufs = [], []
     for l, (buffers, rast, *_) in enumerate(layers):
         if set(buffers) != set(keys):
@@ -478,8 +488,17 @@ def _composite_args(layers, pos, tri, background, topology):
             t = buffers[k]
             what = "layers[%d][%r]" % (l, k)
             check(what, t, dev)
-            if t.dim() != 4 or tuple(t.shape[:3]) != (B, H, W) or t.shape[3] < 1:
+            if spp == 1 and (t.dim() != 4 or tuple(t.shape[:3]) != (B, H, W) or t.shape[3] < 1):
                 raise ValueError("%s: %s must be [%d,%d,%d,C] with C >= 1 like rast, got %s" % (fn, what, B, H, W, tuple(t.shape)))
+            if spp > 1:
+                if t.dim() != 4 or tuple(t.shape[:3]) not in ((B, H, W), (B, Ho, Wo)) or t.shape[3] < 1:
+                    raise ValueError("%s: %s must be [%d,%d,%d,C] (full resolution) or [%d,%d,%d,C] (output resolution) with C >= 1, got %s"
+                                     % (fn, what, B, H, W, B, Ho, Wo, tuple(t.shape)))
+                if res is None:
+                    res = tuple(t.shape[1:3])
+                elif tuple(t.shape[1:3]) != res:
+                    raise ValueError("%s: %s is %s, layers[0][%r] %s: every buffer must be at one resolution"
+                                     % (fn, what, tuple(t.shape), keys[0], tuple(layers[0][0][keys[0]].shape)))
             if cs.setdefault(k, t.shape[3]) != t.shape[3]:
                 raise ValueError("%s: %s has %d channels, layers[0][%r] %d" % (fn, what, t.shape[3], k, cs[k]))
         rasts.append(rast.detach().contiguous())
@@ -501,40 +520,45 @@ def _composite_args(layers, pos, tri, background, topology):
                 raise ValueError("%s: background key %r is not a buffer key" % (fn, k))
             what = "background[%r]" % (k,)
             check(what, t, dev)
-            if tuple(t.shape) != (B, H, W, cs[k]):
-                raise ValueError("%s: %s must be [%d,%d,%d,%d], got %s" % (fn, what, B, H, W, cs[k], tuple(t.shape)))
+            if tuple(t.shape) != (B, Ho, Wo, cs[k]):
+                raise ValueError("%s: %s must be [%d,%d,%d,%d], got %s" % (fn, what, B, Ho, Wo, cs[k], tuple(t.shape)))
             bgs[keys.index(k)] = t
     if topology is not None:
         check("topology", topology, dev, torch.int32)
         if topology.dim() != 2 or topology.shape[1] != 3 or topology.shape[0] != tri.shape[0]:
             raise ValueError("%s: topology must be [T,3] with T = %d like tri, got %s" % (fn, tri.shape[0], tuple(topology.shape)))
-    return keys, rasts, bufs, bgs, pos.contiguous(), tri.contiguous(), topology
+    return keys, rasts, bufs, bgs, pos.contiguous(), tri.contiguous(), topology, spp
 
 
-def composite(layers, pos, tri, background=None, topology=None):
+def composite(layers, pos, tri, background=None, topology=None, spp=1):
     """render_mesh's compositing (the reference's composite_buffer with antialias, render/render.py:284-291, run for every key at
-    :321-330), every buffer of a layer in one launch each way.
+    :321-330, and with spp > 1 the box-filter resolve to the output resolution), every buffer of a layer in one launch each way.
 
     layers: render_mesh's list, front to back, of (buffers, rast[, rast_db]) with buffers a dict of fp32 CUDA [B,H,W,C_k] tensors (any
     strides, C_k >= 1, the same keys and channel counts in every layer, at most 16) and rast that layer's [B,H,W,4] (rast_db is ignored).
     pos the clip-space vertices [V,4] or [B,V,4] and tri int32 [T,3] the layers were rasterised from, as for `antialias`.  background: a
-    dict from key to that key's full [B,H,W,C_k] starting accumulator, e.g. render_mesh's cat((background, zeros)) for 'shaded'; a key
-    without one starts from zeros.  topology: `antialias_topology(tri)`, built inside the call when None.
+    dict from key to that key's starting accumulator at output resolution [B,H/spp,W/spp,C_k], e.g. render_mesh's cat((background,
+    zeros)) for 'shaded'; a key without one starts from zeros.  topology: `antialias_topology(tri)`, built inside the call when None.
 
-    Returns {key: accumulator} for every key: back to front, alpha = (rast.w > 0) * buf[..., -1], accum = antialias(lerp(accum,
-    (buf[..., :-1], 1), alpha)), bit for bit what that torch chain computes with `antialias`.  Differentiable in every buffer (alpha
-    included), in pos and in background.  No host sync; capturable in a CUDA graph when topology is given.  Malformed input raises
-    ValueError naming the argument before any launch.  Semantics: csrc/composite.cu."""
-    keys, rasts, bufs, bgs, pos, tri, topology = _composite_args(layers, pos, tri, background, topology)
+    spp: render_mesh's supersampling factor, an integer >= 1 dividing H and W.  rast stays at full resolution [B,H,W,4]; the buffers are
+    all at full resolution or all at output resolution [B,H/spp,W/spp,C_k] (render_layer with msaa=True), in which case pixel (y, x)
+    reads them at (y // spp, x // spp) as render_layer's nearest upscale would, without making that copy.
+
+    Returns {key: accumulator} for every key at output resolution: back to front, alpha = (rast.w > 0) * buf[..., -1], accum =
+    antialias(lerp(accum, (buf[..., :-1], 1), alpha)), then avg_pool_nhwc(accum, spp) when spp > 1, bit for bit what that torch chain
+    computes with `antialias`.  Differentiable in every buffer (alpha included), in pos and in background.  No host sync; capturable in
+    a CUDA graph when topology is given.  Malformed input raises ValueError naming the argument before any launch.  Semantics:
+    csrc/composite.cu."""
+    keys, rasts, bufs, bgs, pos, tri, topology, spp = _composite_args(layers, pos, tri, background, topology, spp)
     if topology is None:
         topology = antialias_topology(tri)
     topology = topology.contiguous()
     flat = [*rasts, *bgs, *[t for ts in bufs for t in ts]]
     if torch.is_grad_enabled() and (pos.requires_grad or any(t is not None and t.requires_grad for t in flat)):
-        outs = _composite_func.apply(len(keys), len(rasts), pos, tri, topology, *flat)
+        outs = _composite_func.apply(len(keys), len(rasts), spp, pos, tri, topology, *flat)
     else:
         det = lambda t: None if t is None else t.detach()
-        outs, _ = _composite_layers(rasts, [det(t) for t in bgs], [[t.detach() for t in ts] for ts in bufs], pos.detach(), tri, topology,
+        outs, _ = _composite_layers(rasts, [det(t) for t in bgs], [[t.detach() for t in ts] for ts in bufs], pos.detach(), tri, topology, spp,
                                     keep=False)
     return dict(zip(keys, outs))
 

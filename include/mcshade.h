@@ -351,6 +351,22 @@ int mcs_mlptex_fwd(const float *t, int64_t n, const float *aabb, const float *mi
 int mcs_mlptex_bwd(const float *t, int64_t n, const float *aabb, const float *min_max, const float *params, const mcs_hashgrid_levels *lv,
                    int32_t hidden, int32_t channels, const float *const *weights, const float *enc, const float *d_out, float *d_params,
                    float *d_t, float *const *d_weights, void *workspace, mcs_stream stream);
+/* ---- MLP texture pair: MLPTexture3D.sample at each pixel and at its jittered point (render/render.py:63-64) in one forward and one
+ *      backward launch (plus the d W sum); semantics in csrc/mlptexture.cu.  Arguments as mcs_mlptex_fwd / _bwd, n pixels, plus offset [n,3]
+ *      (device fp32, contiguous): the jittered point of pixel i is t_i + offset_i, one fp32 add per component.  out / enc and out_jit /
+ *      enc_jit are the two samples' outputs and encodings, each exactly what mcs_mlptex_fwd gives for t and for t + offset; enc and enc_jit
+ *      are written when non-null, and the backward needs both.  d_out / d_out_jit are the two upstream gradients; either may be null,
+ *      meaning zero.  The backward overwrites d_t [n,3] (may be null) with fl(d_plain + d_jit), and d_offset [n,3] (may be null) with
+ *      d_jit; d_params and d_weights as mcs_mlptex_bwd, d W = fl(d W plain + d W jittered), each summed in chunk order as there.  The
+ *      workspace is 2 x mcs_mlptex_workspace_bytes(n, hidden, channels) bytes.  n = 0 is a no-op (d W zeroed).  No host sync, no
+ *      allocation. */
+int mcs_mlptex_pair_fwd(const float *t, const float *offset, int64_t n, const float *aabb, const float *min_max, const float *params,
+                        const mcs_hashgrid_levels *lv, int32_t hidden, int32_t channels, const float *const *weights, float *out, float *out_jit,
+                        float *enc, float *enc_jit, mcs_stream stream);
+int mcs_mlptex_pair_bwd(const float *t, const float *offset, int64_t n, const float *aabb, const float *min_max, const float *params,
+                        const mcs_hashgrid_levels *lv, int32_t hidden, int32_t channels, const float *const *weights, const float *enc,
+                        const float *enc_jit, const float *d_out, const float *d_out_jit, float *d_params, float *d_t, float *d_offset,
+                        float *const *d_weights, void *workspace, mcs_stream stream);
 
 /* ---- filtered, mip-mapped texture sampling: stands in for nvdiffrast's `dr.texture` in Texture2D.sample and its mip chain's backward
  *      (render/texture.py:27-30,57-68), the regulariser taps (render/render.py:54,75-95) and the probe look-ups (render/light.py:64,76);

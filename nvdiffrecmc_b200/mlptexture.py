@@ -91,6 +91,45 @@ class _mlptex_func(torch.autograd.Function):
         return (d_x, d_p, None, None, None, None, None, *d_w)
 
 
+class _mlptex_pair_func(torch.autograd.Function):
+    """(x, x + off) through the MLP texture in one launch each way; d x = d_plain + d_jit, d off = d_jit, d W = d W plain + d W jit."""
+
+    @staticmethod
+    def forward(ctx, x, off, params, aabb, min_max, lv, hidden, C, *weights):
+        n = x.shape[0]
+        out, out_jit = [torch.empty(n, C, dtype=torch.float32, device=x.device) for _ in range(2)]
+        enc, enc_jit = [torch.empty(n, 32, dtype=torch.float32, device=x.device) for _ in range(2)]
+        _launch_pair_fwd(x, off, params, aabb, min_max, lv, hidden, C, weights, out, out_jit, enc, enc_jit)
+        ctx.save_for_backward(x, off, params, aabb, min_max, enc, enc_jit, *weights)
+        ctx.lv, ctx.hidden, ctx.C = lv, hidden, C
+        ctx.set_materialize_grads(False)          # an unused output's gradient is passed to the kernel as null (zero)
+        return out, out_jit
+
+    @staticmethod
+    def backward(ctx, d_out, d_out_jit):
+        x, off, params, aabb, min_max, enc, enc_jit, *weights = ctx.saved_tensors
+        need_x, need_o, need_p = ctx.needs_input_grad[:3]
+        need_w = list(ctx.needs_input_grad[8:])
+        n, hidden, C = x.shape[0], ctx.hidden, ctx.C
+        d_x = torch.empty_like(x) if need_x else None
+        d_o = torch.empty_like(off) if need_o else None
+        d_p = torch.zeros_like(params) if need_p else None
+        d_w = [torch.zeros_like(w) if nw else None for w, nw in zip(weights, need_w)]
+        if n > 0 and (need_x or need_o or need_p or any(need_w)):
+            ws = None
+            if any(need_w):
+                ws = torch.empty(max(1, 2 * L.lib().mcs_mlptex_workspace_bytes(n, hidden, C) // 4), dtype=torch.float32, device=x.device)
+            g, gj = [d.to(torch.float32).contiguous() if d is not None else None for d in (d_out, d_out_jit)]
+            ptr = lambda v: v.data_ptr() if v is not None else None
+            L.check(L.lib().mcs_mlptex_pair_bwd(x.data_ptr(), off.data_ptr(), n, aabb.data_ptr(), min_max.data_ptr(), params.data_ptr(),
+                                                ctypes.byref(ctx.lv), hidden, C, _ptrs(weights), enc.data_ptr(), enc_jit.data_ptr(), ptr(g),
+                                                ptr(gj), ptr(d_p), ptr(d_x), ptr(d_o), _ptrs(d_w), ptr(ws), L.stream_ptr()),
+                    "mlptex_pair_bwd_dw" if any(need_w) else "mlptex_pair_bwd")
+            if need_p:
+                d_p.mul_(GRADIENT_SCALING)
+        return (d_x, d_o, d_p, None, None, None, None, None, *d_w)
+
+
 def _launch_fwd(x, params, aabb, min_max, lv, hidden, C, weights, out, enc):
     if x.shape[0] == 0:                 # an empty tensor has no storage to point at
         return
@@ -98,9 +137,19 @@ def _launch_fwd(x, params, aabb, min_max, lv, hidden, C, weights, out, enc):
                                    _ptrs(weights), out.data_ptr(), enc.data_ptr() if enc is not None else None, L.stream_ptr()), "mlptex_fwd")
 
 
+def _launch_pair_fwd(x, off, params, aabb, min_max, lv, hidden, C, weights, out, out_jit, enc, enc_jit):
+    if x.shape[0] == 0:
+        return
+    ptr = lambda v: v.data_ptr() if v is not None else None
+    L.check(L.lib().mcs_mlptex_pair_fwd(x.data_ptr(), off.data_ptr(), x.shape[0], aabb.data_ptr(), min_max.data_ptr(), params.data_ptr(),
+                                        ctypes.byref(lv), hidden, C, _ptrs(weights), out.data_ptr(), out_jit.data_ptr(), ptr(enc), ptr(enc_jit),
+                                        L.stream_ptr()), "mlptex_pair_fwd")
+
+
 class MLPTexture3D(torch.nn.Module):
     """The reference's `MLPTexture3D(AABB, channels=3, internal_dims=32, hidden=2, min_max=None)` on the current CUDA device.
-    `sample(texc [..., 3])` -> [..., channels] fp32, differentiable in texc, `encoder.params` and every `net.net` weight."""
+    `sample(texc [..., 3])` -> [..., channels] fp32, differentiable in texc, `encoder.params` and every `net.net` weight.
+    `sample_pair(texc, offset)` -> (sample(texc), sample(texc + offset)) in one launch each way, bit for bit."""
 
     def __init__(self, AABB, channels=3, internal_dims=32, hidden=2, min_max=None):
         super().__init__()
@@ -149,6 +198,32 @@ class MLPTexture3D(torch.nn.Module):
             out = torch.empty(x.shape[0], C, dtype=torch.float32, device=x.device)
             _launch_fwd(x, params, aabb, mm, lv, self.hidden, C, weights, out, None)
         return out.view(*texc.shape[:-1], C)
+
+    def sample_pair(self, texc, offset):
+        """(sample(texc), sample(texc + offset)) -- render.py:63-64's plain and jittered samples of every pixel -- evaluated together:
+        one forward and one backward launch (plus the d W sum), bit for bit the two calls' outputs and their gradients summed by
+        autograd (d texc = d_plain + d_jit, d offset = d_jit, d W = d W plain + d W jit; d params as float atomics, like sample's).
+        texc and offset: [..., 3] of the same shape, floating point, on one device; the jittered point is fp32(texc) + fp32(offset)."""
+        for name, v in (("texc", texc), ("offset", offset)):
+            if not isinstance(v, torch.Tensor) or not v.is_floating_point():
+                raise ValueError("MLPTexture3D.sample_pair: %s must be a floating-point tensor" % name)
+        if texc.shape != offset.shape:
+            raise ValueError("MLPTexture3D.sample_pair: texc %s and offset %s differ in shape" % (tuple(texc.shape), tuple(offset.shape)))
+        if texc.dim() < 1 or texc.shape[-1] != 3:
+            raise ValueError("MLPTexture3D.sample_pair: texc and offset must be [..., 3], got %s" % (tuple(texc.shape),))
+        if offset.device != texc.device:
+            raise ValueError("MLPTexture3D.sample_pair: offset is on %s, texc on %s" % (offset.device, texc.device))
+        aabb, mm, weights = self._operands(texc)
+        x = texc.reshape(-1, 3).to(torch.float32).contiguous()
+        off = offset.reshape(-1, 3).to(torch.float32).contiguous()
+        params, lv, C = self.encoder.params, self.encoder._lv, self.channels
+        if torch.is_grad_enabled() and (x.requires_grad or off.requires_grad or params.requires_grad or any(w.requires_grad for w in weights)):
+            out, out_jit = _mlptex_pair_func.apply(x, off, params, aabb, mm, lv, self.hidden, C, *weights)
+        else:
+            out, out_jit = [torch.empty(x.shape[0], C, dtype=torch.float32, device=x.device) for _ in range(2)]
+            _launch_pair_fwd(x, off, params, aabb, mm, lv, self.hidden, C, weights, out, out_jit, None, None)
+        shape = (*texc.shape[:-1], C)
+        return out.view(shape), out_jit.view(shape)
 
     def clamp_(self):
         pass

@@ -12,6 +12,8 @@ Timed (median of REPS after warm-up):
   sample         MLPTexture3D.sample twice (normalise, clamp, encode, 3 bias-free Linear + ReLU, sigmoid), forward + backward, as the
                  torch composition (encoding kernels + torch MLP) and as the fused drop-in nvdiffrecmc_b200.mlptexture.MLPTexture3D
                  (csrc/mlptexture.cu), the two arms alternated twice; the encode-only composition for scale
+  sample_pair    MLPTexture3D.sample_pair(gb_pos, noise), forward + backward, alternated twice with the fused two-call arm after checking
+                 that the two arms' outputs agree bit for bit; with both arms' launches of our kernels per step (counted by the binding)
   sample_no_grad the fused forward alone under torch.no_grad() at 2048^2 points (render_uv's bake at texture_res)
   torch_*        the same encoding written in plain PyTorch (gather + weighted sum, autograd), the comparison arm; its backward (an
                  accumulating index_put of 128 values per point) takes seconds per call, so it is the median of 3
@@ -106,7 +108,8 @@ def torch_encoding(x, params, lv):
 def run_size(res, raw_only):
     pos, aabb, cov = gbuffer(res)
     gen = torch.Generator(device=dev).manual_seed(0)
-    jit = pos + torch.randn(pos.shape, device=dev, generator=gen) * 0.01
+    noise = torch.randn(pos.shape, device=dev, generator=gen) * 0.01
+    jit = pos + noise
     norm = lambda q: torch.clamp((q.view(-1, 3) - aabb[0][None]) / (aabb[1] - aabb[0])[None], 0, 1).contiguous()
     x = torch.cat([norm(jit), norm(pos)])
     n = x.shape[0]
@@ -167,6 +170,25 @@ def run_size(res, raw_only):
         r["fused_sample_fwd_bwd_ms_%d" % rnd] = event_ms(fused_step, reps=20, label="sample fwd+bwd, fused (round %d)" % rnd)
     r["sample_fwd_bwd_ms"] = min(r["sample_fwd_bwd_ms_0"], r["sample_fwd_bwd_ms_1"])
     r["fused_sample_fwd_bwd_ms"] = min(r["fused_sample_fwd_bwd_ms_0"], r["fused_sample_fwd_bwd_ms_1"])
+    # the pair: both samples of every pixel in one launch each way, the jittered point formed in the kernel from the same noise
+    pq = pos.clone().requires_grad_(True)
+
+    def pair_step():
+        a, b = tex.sample_pair(pq, noise)
+        ((b * g6[0]).sum() + (a * g6[1]).sum()).backward()
+
+    with torch.no_grad():
+        a_p, b_p = tex.sample_pair(pos, noise)
+        if not (torch.equal(a_p, tex.sample(pos)) and torch.equal(b_p, tex.sample(jit))):
+            raise RuntimeError("sample_pair and the two sample calls disagree")
+    for arm, fn in (("fused", fused_step), ("pair", pair_step)):
+        L.LAUNCHES.clear()
+        fn()
+        r["%s_launches_per_step" % arm] = dict(L.LAUNCHES)
+    for rnd in range(2):
+        r["fused_sample_fwd_bwd_ms_pair_round_%d" % rnd] = event_ms(fused_step, reps=20, label="sample fwd+bwd, fused two calls (round %d)" % rnd)
+        r["pair_sample_fwd_bwd_ms_%d" % rnd] = event_ms(pair_step, reps=20, label="sample_pair fwd+bwd (round %d)" % rnd)
+    r["pair_sample_fwd_bwd_ms"] = min(r["pair_sample_fwd_bwd_ms_0"], r["pair_sample_fwd_bwd_ms_1"])
     r["encode_only_fwd_bwd_ms"] = event_ms(lambda: step(False), reps=20, label="encode only fwd+bwd")
     r["mlp_share"] = round(1 - r["encode_only_fwd_bwd_ms"] / r["sample_fwd_bwd_ms"], 3)
     with torch.no_grad():

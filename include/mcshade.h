@@ -197,6 +197,19 @@ int mcs_image_loss_fwd(const mcs_tensor *img, const mcs_tensor *target, int32_t 
 int mcs_image_loss_bwd(const mcs_tensor *img, const mcs_tensor *target, int32_t loss, int32_t tonemapper, const mcs_tensor *d_partials,
                        float *d_img, float *d_target, mcs_stream s);
 
+/* ---- the geometry passes' image loss (geometry/dmtet.py:229-230, geometry/dlmesh.py:75-76): the coverage MSE plus image_loss of the
+ *      colour premultiplied by the target's alpha, mse(img.a, ref.a) + image_loss(img.rgb * ref.a, ref.rgb * ref.a, loss, tonemapper); ids as
+ *      mcs_image_loss_fwd.  img and ref are fp32 [B,H,W,4] views of one B, H, W with any non-negative element strides, B*H*W < 2^31.
+ *      _fwd writes the loss (one float on the device) through `partials`: 2 x mcs_coverage_loss_num_partials(B,H,W) floats of device
+ *      scratch, which hold the per-CTA coverage partials and then the colour partials (the latter equal mcs_image_loss_fwd's of the
+ *      premultiplied colours).  _bwd reads the upstream gradient d_loss (one float on the device) and overwrites d_img, dense [B,H,W,4] and
+ *      16-byte aligned, all four channels; ref is a constant.  Semantics and summation orders in csrc/lossmesh.cu.  No host sync. */
+int mcs_coverage_loss_num_partials(int32_t B, int32_t H, int32_t W);
+int mcs_coverage_loss_fwd(const mcs_tensor *img, const mcs_tensor *ref, int32_t loss, int32_t tonemapper, float *partials, float *loss_out,
+                          mcs_stream s);
+int mcs_coverage_loss_bwd(const mcs_tensor *img, const mcs_tensor *ref, int32_t loss, int32_t tonemapper, const float *d_loss, float *d_img,
+                          mcs_stream s);
+
 /* ---- batched 4x4 transform (row f3): replaces xfm_fwd / xfm_bwd, renderutils/c_src/torch_bindings.cpp:803-864 (mesh.cu:19-90).
  *      points as a (1|B, V, 3, 1) view, matrix as (B, 4, 4, 1); out contiguous [B,V,4] (is_points) or [B,V,3] (vectors);
  *      d_out (B, V, 4|3, 1) view; d_points contiguous [B,V,3] (a broadcast input's gradient is reduced by the caller). */

@@ -139,7 +139,7 @@ LAUNCHES = collections.Counter()
 _KERNELS_PER_CALL = {"optix_build_bvh": 13, "bvh_export": 0, "bvh_export_shadow": 0, "update_pdf": 2, "rasterize": 2, "rasterize_peel": 2,
                      "antialias_topology": 2, "hashgrid_bwd_both": 2, "mlptex_bwd_dw": 2, "mlptex_pair_bwd_dw": 2,
                      "texture_fwd": 1, "texture_bwd": 1, "dmtet_count": 1, "dmtet_emit": 1, "dmtet_bwd": 1, "sdf_reg_fwd": 2, "sdf_reg_bwd": 1,
-                     "shading_loss_fwd": 2, "material_smoothness_grad_fwd": 2, "chroma_loss_fwd": 2,
+                     "shading_loss_fwd": 2, "material_smoothness_grad_fwd": 2, "chroma_loss_fwd": 2, "coverage_loss_fwd": 2,
                      "mip_chain_bwd": 1, "mip_clamp": 1, "mip_normalize": 1, "composite_fwd": 1, "composite_bwd": 1}     # mip_chain_fwd: mcs_mip_chain_fwd_launches(n_levels)
 
 

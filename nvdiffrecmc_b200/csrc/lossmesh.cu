@@ -5,7 +5,29 @@
 //                   torch_bindings.cpp:727-737, has no "n2n" case and silently computes L1 on the CUDA path).
 //   * xfm_points / xfm_vectors : batched 4x4 transform of [1|B, V, 3] points (replaces xfmPointsFwd/BwdKernel,
 //                   render/renderutils/c_src/mesh.cu:19-90, and xfm_fwd/_bwd, torch_bindings.cpp:803-864).
-// Both are HBM-streaming: image_loss reads 24 B/px (fwd) / writes 24 B/px more (bwd); xfm reads 12 B and writes 16 B per vertex.
+//   * coverage_loss : the geometry passes' whole image loss (geometry/dmtet.py:229-230, geometry/dlmesh.py:75-76),
+//                       mse(shaded.a, ref.a) + image_loss(shaded.rgb * ref.a, ref.rgb * ref.a), in one launch each way (+ a one-CTA finish).
+// All are HBM-streaming: image_loss reads 24 B/px (fwd) / writes 24 B/px more (bwd); coverage_loss reads 32 B/px (fwd) and writes 16 B/px
+// more (bwd); xfm reads 12 B and writes 16 B per vertex.
+//
+// coverage_loss contract.  N = B*H*W pixels of shaded and ref ([B,H,W,4] fp32, any strides); per pixel, in fp32:
+//   img_c = shaded_c * ref.a, tgt_c = ref_c * ref.a (c = rgb, each product rounded once, as torch's mul)
+//   colour = image_loss's per-pixel value of (img, tgt): the clamps, the tonemap and loss_fwd1 of k_image_loss_fwd, summed over c, * (1/3)
+//   coverage = (shaded.a - ref.a)^2, the difference and the square each rounded once
+// Forward: CTA k covers pixels [256k, 256k + 256) and sums each term in k_image_loss_fwd's order (butterfly shuffles in each warp, then the
+// eight warp sums in warp order from 0, all fp32); it writes coverage to partials[k] and colour to partials[P + k], P = num_partials.  The
+// colour partials are therefore image_loss's partials of (img, tgt) bit for bit.  The finish (one CTA) sums each half of partials in double,
+// thread t taking partials t, t + 256, ... in index order, then shuffles and warps as above, and writes
+//   loss = fl32(coverage_sum / N + colour_sum / N)          (both quotients and their sum in double, one rounding to fp32)
+// Backward: one thread per pixel reads the upstream gradient G from the device and writes d shaded [B,H,W,4] (dense, 16-byte aligned),
+// every value as autograd forms it through the two torch lines:
+//   rgb:   dv = fl(G * fl(1 / fl32(N))) * (1/3) -- torch's CUDA division of sum(partials) by the host scalar N multiplies by the rounded
+//          reciprocal; the sum passes it to every partial, and k_image_loss_bwd takes a third -- then image_loss's channel backward on
+//          (img_c, tgt_c) and d shaded_c = fl(d img_c * ref.a), mul's backward.
+//   alpha: fl(fl(fl32(2 / N) * fl(shaded.a - ref.a)) * G), mse_loss's backward (alpha * (input - target) * grad, alpha = 2 / numel).
+//   Each value is then added to +0, as autograd adds the two slices' zero-filled gradients: -0 becomes +0.  d ref is not formed.
+// k_image_loss_fwd / _bwd keep their own inline copy of the per-channel loop so that their SASS is what it was; image_loss_px and
+// image_loss_ch_bwd restate it line for line, and tests/test_gpu_coverage_loss.py holds the two to the same bits.
 #include "common.cuh"
 
 namespace {
@@ -128,6 +150,126 @@ __global__ void __launch_bounds__(LOSS_BLOCK) k_image_loss_bwd(LossParams p)
     o2[0] = gt[0]; o2[1] = gt[1]; o2[2] = gt[2];
 }
 
+// ---- coverage_loss (contract in the file header) ----
+// image_loss's per-pixel value, k_image_loss_fwd's loop
+__device__ __forceinline__ float image_loss_px(int loss, int tonemap, const float (&ia)[3], const float (&tb)[3])
+{
+    float v = 0.0f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+        float x = clampf(ia[c], 0.0f, 65535.0f), y = clampf(tb[c], 0.0f, 65535.0f);
+        if (tonemap) { x = fwd_tonemap(x); y = fwd_tonemap(y); }
+        v += loss_fwd1(loss, x, y);
+    }
+    return v * (1.0f / 3.0f);
+}
+
+// d img of one channel, k_image_loss_bwd's loop body (d tgt is not formed)
+__device__ __forceinline__ float image_loss_ch_bwd(int loss, int tonemap, float img, float tgt, float dv)
+{
+    float x = img, y = tgt;
+    if (tonemap) { x = fwd_tonemap(x); y = fwd_tonemap(y); }
+    float di, dt;
+    loss_bwd1(loss, x, y, dv, di, dt);
+    if (tonemap) di = bwd_tonemap(img, di);
+    if (img <= 0.0f || img >= 65535.0f) di = 0.0f;
+    return di;
+}
+
+// sums v[k] over the CTA in k_image_loss_fwd's order; the sums are valid in thread 0
+template <typename T, int K>
+__device__ __forceinline__ void cta_sum(T (&v)[K])
+{
+    __shared__ T s_part[K][LOSS_BLOCK / 32];
+#pragma unroll
+    for (int k = 0; k < K; ++k)
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[k] += __shfl_xor_sync(0xFFFFFFFFu, v[k], o);
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int k = 0; k < K; ++k) s_part[k][threadIdx.x >> 5] = v[k];
+    __syncthreads();
+    if (threadIdx.x == 0)
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            T s = 0;
+#pragma unroll
+            for (int i = 0; i < LOSS_BLOCK / 32; ++i) s += s_part[k][i];
+            v[k] = s;
+        }
+}
+
+struct CoverageParams {
+    TView img, ref;                 // [B,H,W,4]
+    int img_vec, ref_vec;           // dense and 16-byte aligned: one float4 per pixel
+    int H, W; int64_t npx;
+    int loss, tonemap;
+    float *partial;                 // fwd: [2P], coverage then colour
+    const float *d_loss;            // bwd: G, one float
+    float inv_npx, two_over_npx;    // bwd: fl32(1 / fl32(N)), fl32(2 / N)
+    float *d_img;                   // bwd: dense [B,H,W,4]
+};
+
+__device__ __forceinline__ float4 ld_rgba(const TView &v, int vec, int64_t px, int n, int h, int w)
+{
+    if (vec) return __ldg(reinterpret_cast<const float4 *>(v.p) + px);
+    const float *q = v.p + v.off(n, h, w);
+    return make_float4(__ldg(q), __ldg(q + v.s3), __ldg(q + 2 * v.s3), __ldg(q + 3 * v.s3));
+}
+
+__device__ __forceinline__ void premultiply(float4 s, float4 r, float (&ia)[3], float (&tb)[3])
+{
+    ia[0] = __fmul_rn(s.x, r.w); ia[1] = __fmul_rn(s.y, r.w); ia[2] = __fmul_rn(s.z, r.w);
+    tb[0] = __fmul_rn(r.x, r.w); tb[1] = __fmul_rn(r.y, r.w); tb[2] = __fmul_rn(r.z, r.w);
+}
+
+__global__ void __launch_bounds__(LOSS_BLOCK) k_coverage_loss_fwd(CoverageParams p)
+{
+    const int64_t px = (int64_t)blockIdx.x * LOSS_BLOCK + threadIdx.x;
+    float v[2] = {0.0f, 0.0f};                                  // coverage, colour
+    if (px < p.npx) {
+        const int w = (int)(px % p.W); const int64_t t = px / p.W; const int h = (int)(t % p.H), n = (int)(t / p.H);
+        const float4 s = ld_rgba(p.img, p.img_vec, px, n, h, w), r = ld_rgba(p.ref, p.ref_vec, px, n, h, w);
+        float ia[3], tb[3];
+        premultiply(s, r, ia, tb);
+        const float e = __fsub_rn(s.w, r.w);
+        v[0] = __fmul_rn(e, e);
+        v[1] = image_loss_px(p.loss, p.tonemap, ia, tb);
+    }
+    cta_sum(v);
+    if (threadIdx.x == 0) {
+        p.partial[blockIdx.x] = v[0];
+        p.partial[gridDim.x + blockIdx.x] = v[1];
+    }
+}
+
+__global__ void __launch_bounds__(LOSS_BLOCK) k_coverage_loss_finish(const float *__restrict__ part, int nparts, int64_t npx, float *__restrict__ loss)
+{
+    double v[2] = {0.0, 0.0};
+    for (int i = threadIdx.x; i < nparts; i += LOSS_BLOCK) {
+        v[0] += (double)part[i];
+        v[1] += (double)part[nparts + i];
+    }
+    cta_sum(v);
+    if (threadIdx.x == 0) *loss = (float)(v[0] / (double)npx + v[1] / (double)npx);
+}
+
+__global__ void __launch_bounds__(LOSS_BLOCK) k_coverage_loss_bwd(CoverageParams p)
+{
+    const int64_t px = (int64_t)blockIdx.x * LOSS_BLOCK + threadIdx.x;
+    if (px >= p.npx) return;
+    const int w = (int)(px % p.W); const int64_t t = px / p.W; const int h = (int)(t % p.H), n = (int)(t / p.H);
+    const float G = __ldg(p.d_loss);
+    const float dv = __fmul_rn(G, p.inv_npx) * (1.0f / 3.0f);
+    const float4 s = ld_rgba(p.img, p.img_vec, px, n, h, w), r = ld_rgba(p.ref, p.ref_vec, px, n, h, w);
+    float ia[3], tb[3], g[3];
+    premultiply(s, r, ia, tb);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) g[c] = __fadd_rn(__fmul_rn(image_loss_ch_bwd(p.loss, p.tonemap, ia[c], tb[c], dv), r.w), 0.0f);
+    const float ga = __fadd_rn(__fmul_rn(__fmul_rn(p.two_over_npx, __fsub_rn(s.w, r.w)), G), 0.0f);
+    reinterpret_cast<float4 *>(p.d_img)[px] = make_float4(g[0], g[1], g[2], ga);
+}
+
 struct XfmParams {
     const float *points; int p_s0, p_s1, p_s2; int p_b;     // [1|B, V, 3]
     const float *matrix; int m_s0, m_s1, m_s2;              // [B, 4, 4]
@@ -196,6 +338,35 @@ static int loss_common(LossParams &p, const mcs_tensor *img, const mcs_tensor *t
     return 0;
 }
 
+static bool dense_rgba(const mcs_tensor *t)
+{
+    const int32_t *sz = t->sizes, *st = t->strides;
+    return ((uintptr_t)t->ptr & 15) == 0 && st[3] == 1 && (sz[2] == 1 || st[2] == 4) && (sz[1] == 1 || st[1] == 4 * sz[2]) &&
+           (sz[0] == 1 || (int64_t)st[0] == 4 * (int64_t)sz[1] * sz[2]);
+}
+
+static int coverage_common(const char *fn, CoverageParams &p, const mcs_tensor *img, const mcs_tensor *ref, int32_t loss, int32_t tonemapper)
+{
+    MCS_REQUIRE(loss >= 0 && loss <= 4, "%s: unknown loss id %d (0 l1, 1 mse, 2 relmse, 3 smape, 4 n2n)", fn, loss);
+    MCS_REQUIRE(tonemapper == 0 || tonemapper == 1, "%s: unknown tonemapper id %d (0 none, 1 log_srgb)", fn, tonemapper);
+    const mcs_tensor *v[2] = {img, ref};
+    const char *names[2] = {"img", "ref"};
+    for (int i = 0; i < 2; ++i) {
+        MCS_REQUIRE(v[i] && v[i]->ptr, "%s: %s is null", fn, names[i]);
+        MCS_REQUIRE(v[i]->sizes[3] == 4, "%s: %s must have 4 channels, got %d", fn, names[i], v[i]->sizes[3]);
+        for (int d = 0; d < 3; ++d) MCS_REQUIRE(v[i]->sizes[d] == img->sizes[d], "%s: ref must have the shape of img", fn);
+        for (int d = 0; d < 4; ++d) MCS_REQUIRE(v[i]->strides[d] >= 0, "%s: %s has a negative stride", fn, names[i]);
+    }
+    MCS_REQUIRE(img->sizes[0] > 0 && img->sizes[1] > 0 && img->sizes[2] > 0, "%s: empty operands", fn);
+    p.npx = (int64_t)img->sizes[0] * img->sizes[1] * img->sizes[2];
+    MCS_REQUIRE(p.npx < (int64_t)1 << 31, "%s: %lld pixels, at most 2^31 - 1", fn, (long long)p.npx);
+    p.H = img->sizes[1]; p.W = img->sizes[2];
+    p.img = make_view(img); p.ref = make_view(ref);
+    p.img_vec = dense_rgba(img); p.ref_vec = dense_rgba(ref);
+    p.loss = loss; p.tonemap = tonemapper;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -225,6 +396,38 @@ int mcs_image_loss_bwd(const mcs_tensor *img, const mcs_tensor *target, int32_t 
     p.dout = make_view(d_partials); p.dout_n = d_partials->sizes[0];
     p.d_img = d_img; p.d_tgt = d_target;
     k_image_loss_bwd<<<nb, LOSS_BLOCK, 0, (cudaStream_t)s>>>(p);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_coverage_loss_num_partials(int32_t B, int32_t H, int32_t W) { return mcs_image_loss_num_partials(B, H, W); }
+
+int mcs_coverage_loss_fwd(const mcs_tensor *img, const mcs_tensor *ref, int32_t loss, int32_t tonemapper, float *partials, float *loss_out,
+                          mcs_stream s)
+{
+    CoverageParams p{};
+    if (int e = coverage_common("coverage_loss_fwd", p, img, ref, loss, tonemapper)) return e;
+    MCS_REQUIRE(partials && loss_out, "coverage_loss_fwd: null output pointer");
+    p.partial = partials;
+    const int nb = mcs_coverage_loss_num_partials(img->sizes[0], p.H, p.W);
+    k_coverage_loss_fwd<<<nb, LOSS_BLOCK, 0, (cudaStream_t)s>>>(p);
+    MCS_LAUNCH_CHECK();
+    k_coverage_loss_finish<<<1, LOSS_BLOCK, 0, (cudaStream_t)s>>>(partials, nb, p.npx, loss_out);
+    MCS_LAUNCH_CHECK();
+    return 0;
+}
+
+int mcs_coverage_loss_bwd(const mcs_tensor *img, const mcs_tensor *ref, int32_t loss, int32_t tonemapper, const float *d_loss, float *d_img,
+                          mcs_stream s)
+{
+    CoverageParams p{};
+    if (int e = coverage_common("coverage_loss_bwd", p, img, ref, loss, tonemapper)) return e;
+    MCS_REQUIRE(d_loss && d_img, "coverage_loss_bwd: null pointer argument");
+    MCS_REQUIRE(((uintptr_t)d_img & 15) == 0, "coverage_loss_bwd: d_img must be 16-byte aligned");
+    p.d_loss = d_loss; p.d_img = d_img;
+    p.inv_npx = 1.0f / (float)p.npx;
+    p.two_over_npx = (float)(2.0 / (double)p.npx);
+    k_coverage_loss_bwd<<<mcs_coverage_loss_num_partials(img->sizes[0], p.H, p.W), LOSS_BLOCK, 0, (cudaStream_t)s>>>(p);
     MCS_LAUNCH_CHECK();
     return 0;
 }

@@ -1,7 +1,9 @@
 """The image-space regularisers of both geometry passes on the GPU: drop-ins for the reference's `shading_loss`,
 `material_smoothness_grad` and `chroma_loss` (render/regularizer.py:15-49), run by the kernels of csrc/regularizer.cu (contract stated
 there: torch's conventions for ties of max, clamp boundaries, abs at 0, the sRGB branch and the means' denominators), and
-`jitter_taps`, the producer of their inputs in shade() (render/render.py:50-97), run by the kernels of csrc/taps.cu.
+`jitter_taps`, the producer of their inputs in shade() (render/render.py:50-97), run by the kernels of csrc/taps.cu, and
+`coverage_image_loss`, the image loss the geometry passes put in front of them (geometry/dmtet.py:229-230, geometry/dlmesh.py:75-76): the
+coverage MSE plus `image_loss` of the colour premultiplied by the target's alpha, run by the kernels of csrc/lossmesh.cu.
 
 Each function returns a 0-dim fp32 device tensor, as `torch.mean(...) * lambda` does.  Forward and backward are one streaming launch
 each (plus a one-CTA finish in the forward), make no host synchronisation and can be captured in a CUDA graph; the backward reads its
@@ -10,13 +12,15 @@ depends on the geometry); `kd`'s alpha gets exactly 0 and `color_ref` is the con
 
 Operands are fp32 CUDA [B,H,W,4] tensors of one B, H, W, with any strides (`color_ref` is often a slice); `material_smoothness_grad`'s
 kd_grad may also be [B,H,W,5], the transparency configuration's 4-channel kd with alpha appended.  A wrong channel count, a shape
-mismatch, a CPU tensor, a non-float lambda or a `color_ref` that requires grad raises ValueError before anything is launched.
+mismatch, a CPU tensor, a non-float lambda or a `color_ref` that requires grad raises ValueError before anything is launched, as does
+an unknown loss or tonemapper name for `coverage_image_loss`.
 """
 import torch
 
 from . import _lib as L
+from .renderutils.ops import _loss_ids
 
-__all__ = ["shading_loss", "material_smoothness_grad", "chroma_loss", "jitter_taps"]
+__all__ = ["shading_loss", "material_smoothness_grad", "chroma_loss", "jitter_taps", "coverage_image_loss"]
 
 
 def _check(fn, named, lambdas, chans=None):
@@ -269,3 +273,44 @@ def jitter_taps(rast, jitter, kd, ks, gb_normal, perturbed_nrm=None, kd_jitter=N
         outs = _taps_fwd(tuple(None if t is None else t.detach() for t in ops))
     names = ["kd_grad", "ks_grad", "normal_grad", "perturbed_nrm_grad"]
     return dict(zip(names, outs))
+
+
+# ---- coverage_image_loss ----
+def _coverage_fwd(s, r, ids):
+    B, H, W = s.shape[:3]
+    loss = torch.empty((), dtype=torch.float32, device=s.device)
+    partials = torch.empty(2 * L.lib().mcs_coverage_loss_num_partials(B, H, W), dtype=torch.float32, device=s.device)
+    L.check(L.lib().mcs_coverage_loss_fwd(L.nhwc(s), L.nhwc(r), *ids, partials.data_ptr(), loss.data_ptr(), L.stream_ptr()), "coverage_loss_fwd")
+    return loss
+
+
+class _CoverageImageLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, s, r, ids):
+        ctx.save_for_backward(s, r)
+        ctx.ids = ids
+        return _coverage_fwd(s, r, ids)
+
+    @staticmethod
+    def backward(ctx, d_loss):
+        if not ctx.needs_input_grad[0]:
+            return None, None, None
+        s, r = ctx.saved_tensors
+        gs = _grad(s)
+        L.check(L.lib().mcs_coverage_loss_bwd(L.nhwc(s), L.nhwc(r), *ctx.ids, _upstream(d_loss).data_ptr(), gs.data_ptr(), L.stream_ptr()),
+                "coverage_loss_bwd")
+        return gs, None, None
+
+
+def coverage_image_loss(shaded, color_ref, loss='l1', tonemapper='none'):
+    """The geometry passes' image loss (geometry/dmtet.py:229-230, geometry/dlmesh.py:75-76):
+        mse_loss(shaded[..., 3:], color_ref[..., 3:]) + image_loss(shaded[..., 0:3] * color_ref[..., 3:], color_ref[..., 0:3] * color_ref[..., 3:],
+                                                                   loss, tonemapper)
+    with `image_loss` the package's renderutils op (so 'n2n' is honoured) and loss / tonemapper one of train.py's createLoss pairs.  The
+    first term is the silhouette loss: shaded's alpha is the composited coverage.  -> 0-dim fp32 tensor, differentiable in all four
+    channels of shaded; color_ref is the constant target."""
+    ids = _loss_ids(loss, tonemapper)
+    _check("coverage_image_loss", [("shaded", shaded), ("color_ref", color_ref)], [])
+    if torch.is_grad_enabled() and shaded.requires_grad:
+        return _CoverageImageLoss.apply(shaded, color_ref, ids)
+    return _coverage_fwd(shaded.detach(), color_ref, ids)
